@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — LM iterations/sec of the ITERATIVE_SCHUR + SCHUR_JACOBI bundle-adjustment hot path.
 
-  python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl b200|reference]
+  python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl b200|reference] [--dump-outputs DIR]
 
 A "step" is one Levenberg-Marquardt iteration (ComputeTrustRegionStep: LM diagonal, implicit-Schur PCG solve,
 model cost; candidate cost evaluation; on acceptance a Jacobian evaluation + column scaling) of the configuration
@@ -14,6 +14,10 @@ steps on the same problem (the state is reset in between, so every timed run doe
              (state/D/residual/step copies inside the timed region)
   roofline   dominant kernel: algorithmic bytes per launch / mean CUDA-event time per launch, vs measured HBM peak
   cpu_baseline / --impl reference: the CPU restatement of the reference path (oracle/) on the host cores
+
+--dump-outputs DIR writes what the timed run returned to its caller as DIR/<name>.npy (float64): the final state
+(points then cameras, reduced-program order; rank 0's shard when sharded) and the per-iteration trace, so that two
+builds can be compared output for output on identical seeded inputs.  For spmv-sweep: the products of the largest size.
 """
 import argparse
 import json
@@ -28,16 +32,25 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+DUMP_BYTES = 60_000_000   # --dump-outputs budget over all arrays
 
 
-def ncu_traffic(workload, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the kernel on this workload, from the committed
-    `ncu --set full` captures (profiles/ncu_traffic.json, written by tools/ncu_summary.py); None if never captured."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(workload, {}).get(kernel)
-    except Exception:
-        return None
+def dump_outputs(path, arrays):
+    """Writes every array as path/<name>.npy in float64.  When they exceed DUMP_BYTES together, each array larger than
+    an equal share is replaced by a fixed sample of that share (indices from RandomState(0), sorted), the same for every
+    build and run."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: np.ascontiguousarray(v, dtype=np.float64).ravel() for k, v in arrays.items()}
+    share = DUMP_BYTES // (8 * len(arrays))
+    sample = 8 * sum(a.size for a in arrays.values()) > DUMP_BYTES
+    for name, a in arrays.items():
+        if sample and a.size > share:
+            a = a[np.sort(np.random.RandomState(0).randint(0, a.size, share))]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
+def trace_arrays(recs):
+    return {k: np.array([float(r[k]) for r in recs]) for k in ("cost", "step_norm", "gradient_max_norm", "ls_iterations")}
 
 
 def op_rate(v, peak):
@@ -59,7 +72,7 @@ def load_peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s)"
 
 
 def make_problem(workload):
@@ -129,7 +142,7 @@ def make_config(desc, num_obs):
     jb = 192 * num_obs
     return {"workload": desc, "linear_solver": "ITERATIVE_SCHUR", "preconditioner": "SCHUR_JACOBI", "eta": 1e-2,
             "max_linear_solver_iterations": 500, "jacobian_bytes": jb,
-            "l2": "inputs larger than L2 (J alone is %.0f MB)" % (jb / 1e6) if jb > 126e6
+            "l2": "inputs larger than L2 (J alone is %.0f MB)" % (jb / 1e6) if jb > 50e6
             else "working set fits L2: roofline fraction is vs HBM peak and may exceed 1"}
 
 
@@ -149,10 +162,11 @@ def run_reference(args, bal, desc, rank0=True):
         ow.max_num_iterations = 1
         prog.solve(state, ow)
     t0 = time.perf_counter()
-    _, recs, times = prog.solve(state, o)
+    state_out, recs, times = prog.solve(state, o, max_records=args.steps + 1)
     dt = time.perf_counter() - t0
     iters = max(1, len(recs) - 1)
-    return {"value": iters / dt, "seconds": dt, "iterations": iters, "cores": nt, "trace": recs, "times": times}
+    return {"value": iters / dt, "seconds": dt, "iterations": iters, "cores": nt, "trace": recs, "times": times,
+            "state": state_out}
 
 
 def run_spmv_sweep(args):
@@ -186,18 +200,15 @@ def run_spmv_sweep(args):
         reps = 5 if N <= 3_000_000 else 2
 
         def ops():
-            gpu.partitioned_multiply(0, x[:3 * P])
-            gpu.partitioned_multiply(2, y)
-            gpu.partitioned_multiply(1, x[3 * P:])
-            gpu.partitioned_multiply(3, y)
-            gpu.right_multiply(x)
-            gpu.left_multiply(y)
-            gpu.jtj_multiply(x, D)
+            return {"pmv_right_e": gpu.partitioned_multiply(0, x[:3 * P]), "pmv_left_e": gpu.partitioned_multiply(2, y),
+                    "pmv_right_f": gpu.partitioned_multiply(1, x[3 * P:]), "pmv_left_f": gpu.partitioned_multiply(3, y),
+                    "jacobian_multiply": gpu.right_multiply(x), "jacobian_t_multiply": gpu.left_multiply(y),
+                    "jtj_multiply": gpu.jtj_multiply(x, D)}
         ops()   # warm-up
         gpu.stats_reset()
         gpu.profile(True)
         for _ in range(reps):
-            ops()
+            out = ops()
         st = gpu.stats()
         gpu.profile(False)
         row = {"N": N, "P": P, "C": C, "jacobian_bytes": 192 * N, "ops": {}}
@@ -206,6 +217,9 @@ def run_spmv_sweep(args):
             if r:
                 row["ops"][label] = {"GBps": r["GBps"], "frac": r["frac"], "mean_op_ms": r["mean_op_ms"]}
         rows.append(row)
+        if args.dump_outputs and N == sizes[-1] - sizes[-1] % 4:
+            dump_outputs(args.dump_outputs, out)
+        del out
         gpu.close()
         torch.cuda.empty_cache()
     last = rows[-1]["ops"].get("(J'J + D^2) x", {})
@@ -226,7 +240,11 @@ def main():
     ap.add_argument("--workload", default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--sizes", default=None, help="spmv-sweep: comma separated N list (default 1e5..3e7; 1e8 needs ~60 GB host RAM)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed run as DIR/<name>.npy (float64, <= 60 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -253,6 +271,8 @@ def main():
                                  "sample": "%d LM iterations from the initial point, %d CG iterations" % (
                                      r["iterations"], sum(int(t["ls_iterations"]) for t in r["trace"]))},
                 "e2e": {"value": r["value"], "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dict(state=r["state"], **trace_arrays(r["trace"])))
         print(json.dumps(line))
         return 0
 
@@ -295,7 +315,8 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0 = time.perf_counter()
         e0.record(stream)
-        _, recs = gpu.lm_solve(state0, gpu.lm_options(max_num_iterations=iters), host_boundary=host_boundary)
+        state, recs = gpu.lm_solve(state0, gpu.lm_options(max_num_iterations=iters), host_boundary=host_boundary,
+                                   max_records=iters + 1)
         e1.record(stream)
         torch.cuda.synchronize()
         wall = time.perf_counter() - t0
@@ -305,7 +326,7 @@ def main():
             t = torch.tensor([dev, wall], dtype=torch.float64, device="cuda")
             dist.all_reduce(t, op=dist.ReduceOp.MAX)   # max over ranks
             dev, wall = float(t[0]), float(t[1])
-        return dev, wall, recs
+        return dev, wall, recs, state
 
     # warm-up
     single = world == 1
@@ -315,14 +336,14 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     gpu.stats_reset()
-    dev_s, wall_s, recs = timed_solve(args.steps, False)
+    dev_s, wall_s, recs, state_out = timed_solve(args.steps, False)
     launches = gpu.total_launches()
     clocks = sampler.stop()
     iters = max(1, len(recs) - 1)
     # end to end through the host-buffer boundary (N > 1: every rank drives its shard through the same entry points with its
     # own host buffers; the few host-side scalars of the loop are combined across ranks; wall clock, max over ranks)
     gpu.stats_reset()
-    e2e_dev_s, e2e_wall_s, recs_e2e = timed_solve(args.steps, True)
+    e2e_dev_s, e2e_wall_s, recs_e2e, _ = timed_solve(args.steps, True)
     h2d, d2h = gpu.transfer_bytes()
     e2e_iters = max(1, len(recs_e2e) - 1)
     # per-kernel event timing for the roofline (same steps, instrumented)
@@ -397,7 +418,7 @@ def main():
                     "d2h_bytes_per_step": d2h // e2e_iters, "device_seconds": e2e_dev_s, "wall_seconds": e2e_wall_s},
             "gpu_launches": launches, "clocks": clocks, "wall_seconds": wall_s,
             "roofline": {"bound": "hbm", "kernel": dom_name, "achieved": dom["GBps"], "peak": peak, "unit": "GB/s",
-                         "frac": dom["frac"], "traffic": ncu_traffic(workload, dom_name), "peak_source": peak_src,
+                         "frac": dom["frac"], "peak_source": peak_src,
                          "bytes_per_operation": dom["bytes_per_operation"], "operations": dom["operations"],
                          "launches": dom["launches"], "dominant_kernel_by_time": by_time,
                          "mean_op_ms": dom["mean_op_ms"],
@@ -419,6 +440,8 @@ def main():
         line["cpu_baseline"] = {"value": r["value"], "unit": UNIT, "cores": r["cores"], "kind": "port",
                                 "sample": "%d LM iterations from the same initial point (%d CG iterations), %.1f s" % (
                                     r["iterations"], sum(int(t["ls_iterations"]) for t in r["trace"]), r["seconds"])}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dict(state=state_out, **trace_arrays(recs)))
     print(json.dumps(line))
     gpu.close()
     if world > 1:

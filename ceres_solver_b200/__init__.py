@@ -1,4 +1,4 @@
-"""ceres_solver_b200 — B200-native (sm_100a) implementation of Ceres Solver's Levenberg-Marquardt inner-loop
+"""ceres_solver_b200 — H100-native (sm_90a) implementation of Ceres Solver's Levenberg-Marquardt inner-loop
 hot path for bundle adjustment: CUDA kernels + C ABI in csrc/ (libb200ba.so), ctypes plumbing in binding.py,
 host-side problem preparation in bal.py.  No CPU fallback: using the compute path without the built library
 or without a GPU raises."""

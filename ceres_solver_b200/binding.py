@@ -114,7 +114,7 @@ def _check(rc):
         raise B200Error(rc, lib().b200_last_error().decode())
 
 
-def plan_point_order(num_cameras, num_points, cam_idx, pt_idx, num_chunks=148):
+def plan_point_order(num_cameras, num_points, cam_idx, pt_idx, num_chunks=132):
     """Host-only: the internal point order b200_create would choose.  Returns (perm, metrics[4], choice)."""
     cam = np.ascontiguousarray(cam_idx, dtype=np.int32)
     pt = np.ascontiguousarray(pt_idx, dtype=np.int32)

@@ -1,6 +1,6 @@
 // libb200ba.so — host side of the C ABI declared in include/b200ba.h.
 //
-// Owns the device-resident bundle adjustment problem (SURVEY Appendix B layout), launches the sm_100a
+// Owns the device-resident bundle adjustment problem (SURVEY Appendix B layout), launches the sm_90a
 // kernels of kernels.cuh / vector_kernels.cuh on one stream, and implements
 //   * the Evaluator-shaped entry points   (internal/ceres/evaluator.h:60-168),
 //   * the SparseMatrix-shaped entry points on the device Jacobian (internal/ceres/sparse_matrix.h:67-116),
@@ -208,7 +208,7 @@ struct b200_handle {
   cudaStream_t stream2 = nullptr;   // side stream for the big-point kernel inside the PCG
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool own_stream = false;
-  int sm_count = 148;
+  int sm_count = 132;
   int C = 0, P = 0, N = 0, num_tiles = 0;
   int np = 0;  // 3P + 9C
   int loss_type = 0;
@@ -1327,8 +1327,8 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   CU(cudaSetDevice(desc->device));
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, desc->device));
-  if (prop.major < 10)
-    return fail(B200_ERR_NO_DEVICE, "device %s is sm_%d%d; this library is built for sm_100a only", prop.name, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)   // sm_90a code loads on sm_90 devices only
+    return fail(B200_ERR_NO_DEVICE, "device %s is sm_%d%d; this library is built for sm_90a (H100) only", prop.name, prop.major, prop.minor);
 
   const int C = desc->num_cameras, P = desc->num_points;
   const int N = static_cast<int>(desc->num_observations);
@@ -1488,7 +1488,7 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   if (v2_possible && !wtiles.empty()) {
     // Static partition by position in the row order, balanced by cost: a warp tile costs about the same whatever its
     // fill (the kernels are bound by warp-instruction issue / LSU work, not by bytes), and a >32-row point, which the
-    // whole CTA processes serially, costs as much as ~20 tiles (in-kernel time stamps, profiles/r01_pcg_persistent_trace_l1723.txt).
+    // whole CTA processes serially, costs as much as ~20 tiles (in-kernel time stamps).
     // CTA b owns the items whose cumulative cost starts in [total * b / n, total * (b + 1) / n): neighbouring CTAs stream
     // neighbouring HBM ranges and touch neighbouring cameras.
     const int T = static_cast<int>(wtiles.size());
@@ -1559,8 +1559,8 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
         max_list = std::max(max_list, static_cast<int>(lists[b].size()));
         max_range = std::max(max_range, hi - lo);
       }
-      // <= ~4 us of REDs at the measured 95 G lane-RED/s; list positions must fit the row word
-      long direct_limit = 700000;   // REDs of the flush: <= ~7 us at the measured 95 G lane-RED/s, still far cheaper than partial vectors
+      // list positions must fit the row word
+      long direct_limit = 700000;   // REDs of the flush: a few microseconds, still far cheaper than partial vectors
       if (const char* e = dev_env("B200_DIRECT_LIMIT")) direct_limit = atol(e);
       direct_mode = 9 * list_total <= direct_limit && max_list <= static_cast<int>(kMetaLocalMask) && C <= static_cast<int>(kMetaCamMask);
       if (C > static_cast<int>(kMetaCamMask)) v2_possible = false;   // camera ids do not fit the row word: CTA-tile kernels

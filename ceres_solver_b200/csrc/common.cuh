@@ -1,5 +1,5 @@
 // Device-side plumbing shared by every tile kernel of libb200ba: the HBM-resident problem layout,
-// TMA (cp.async.bulk) + mbarrier wrappers for sm_100a, and the per-tile bookkeeping.
+// TMA (cp.async.bulk) + mbarrier wrappers for sm_90a, and the per-tile bookkeeping.
 //
 // Layout in HBM (SURVEY Appendix B; reference origin in brackets):
 //   values      [24N] f64   all E cells [N][2][3] then all F cells [N][2][9]   (block_jacobian_writer.cc:68-167)

@@ -6,7 +6,7 @@
 // (ChunkOuterProduct, :519-568); here one CTA takes a point, stages W_r = E_r'F_r (3x9) and P W_r for 96 rows at a time
 // in shared memory and every thread walks the (r, s) pairs of the two staged slices, adding W_r' (P W_s) into the block
 // (cam_r, cam_s) of the LOWER triangle (cam_r >= cam_s; column-major for cuSOLVER) with FP64 REDs -- the assembly is bound
-// by the ~95 G RED/s of the device (81 per pair), ~3 ms on Ladybug-1723.  The diagonal blocks also receive F_r'F_r.
+// by the device's FP64 RED rate (81 per pair).  The diagonal blocks also receive F_r'F_r.
 #pragma once
 #include "kernels.cuh"
 

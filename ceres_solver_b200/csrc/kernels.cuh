@@ -1,4 +1,4 @@
-// Tile kernels of libb200ba (sm_100a).  One CTA processes one tile (<= kTile rows = whole points) per
+// Tile kernels of libb200ba (sm_90a).  One CTA processes one tile (<= kTile rows = whole points) per
 // loop iteration; E/F cells are staged into shared memory by TMA bulk copies (UBLKCP) and read back with
 // conflict-free 128-bit LDS; per-point quantities are reduced in shared memory inside the tile (points never
 // straddle tiles, so there is no cross-CTA traffic for the e blocks); camera-sized results are accumulated

@@ -1,9 +1,8 @@
-// Warp-tile kernels (v2): the camera-scatter kernels re-designed around what the B200 measurements say
-// (profiles/r01_microbench_atomics_gather_stream.txt):
-//   * FP64 global RED tops out at ~95 G lane-ops/s chip-wide, regardless of locality -> 9 REDs per row make
-//     S*x RED-bound at ~29 % of the HBM roofline (profiles/r01_v1_schur_mul_ncu_details.txt);
-//   * FP64 atomics on SHARED memory (ATOMS.CAST.SPIN.64) sustain ~430 G lane-ops/s;
-//   * a TMA bulk-copy ring streams HBM at 7.2 TB/s.
+// Warp-tile kernels (v2): the camera-scatter kernels built around three properties of the memory system:
+//   * FP64 global REDs have a chip-wide rate limit regardless of locality -> 9 REDs per row make S*x RED-bound far
+//     below the HBM roofline;
+//   * FP64 atomics on SHARED memory (ATOMS.CAST.SPIN.64) sustain several times that rate;
+//   * a TMA bulk-copy ring streams HBM close to its peak.
 // So: one persistent CTA per SM keeps a PRIVATE copy of the camera-sized output in shared memory, rows are
 // processed in warp-sized tiles (whole points, <= 32 rows) so that the per-point reduction needs only
 // __syncwarp (no CTA barrier anywhere in the main loop), every warp runs its own TMA ring for the 2x9 F
@@ -164,9 +163,9 @@ __device__ __forceinline__ void v2_epilogue(const V2View& v, const double* sy, i
 // Accumulate one 9-vector per row into the CTA-private camera vector.
 //  1. rows of the warp that hit the same camera are summed through shuffles first (binary tree over the rank inside
 //     each __match_any group): with the camera locality of real captures a warp tile touches a handful of cameras,
-//     and un-aggregated lanes would fight over the same shared-memory words (measured: 3x slower than random data);
+//     and un-aggregated lanes would fight over the same shared-memory words;
 //  2. the group leaders add into replica `rep` of the vector (one replica per warp when shared memory allows, so
-//     different warps never collide) with shared-memory FP64 atomics (ATOMS.CAST.SPIN.64, ~430 G lane-ops/s).
+//     different warps never collide) with shared-memory FP64 atomics (ATOMS.CAST.SPIN.64).
 __device__ __forceinline__ void cam_accumulate9(double* sy_rep, int cam_local, bool active, double (&g)[9]) {
   const int lane = threadIdx.x & 31;
   const int key = active ? cam_local : (0x40000000 | lane);
@@ -454,8 +453,7 @@ __global__ void __launch_bounds__(kV3MaxThreads, 1)
 // v4: every operand of a warp tile arrives through the warp's TMA ring -- the 2x9 F cells, the 2x3 E cells, the
 // (E'E+D^2)^-1 blocks of its points and a 160-byte descriptor block (row words, the tile's own extents and the extents
 // of the tile that will reuse the ring slot) -- and x of the CTA's camera range is staged once in shared memory, so the
-// main loop issues no global load at all (ncu on v3, profiles/r01_v3_schur_mul_l1723_ncu.txt: a third of all stall
-// samples were long-scoreboard waits on the row word -> x -> (E'E)^-1 dependency chain).  The slot's contents go to
+// main loop issues no global load at all (no long-scoreboard waits on the row word -> x -> (E'E)^-1 dependency chain).  The slot's contents go to
 // registers first (the F cells stay there, 36 registers; the kernel sits at 122-126 of the 128 registers that 16 warps
 // allow) and the slot is refilled at once, so one slot per warp is enough; with one private camera vector per warp the
 // accumulation needs no atomics (cam_accumulate9_owned).
@@ -687,7 +685,7 @@ __device__ __forceinline__ void v4_tiles(const V2View& v, const double* ete_inv,
       w2 = e1.x * t0 + e2.y * t1;
     }
     // u = sum over the rows of the point of E'(F x): segmented suffix sums by shuffles (log2(longest point of the tile)
-    // steps; measured 6-8 % faster than the exchange through shared memory: the kernel is bound by LSU wavefronts), the
+    // steps, fewer LSU wavefronts than an exchange through shared memory), the
     // total sits in the point's first lane and is broadcast from there
     seg_suffix_sum3(w0, w1, w2, sg.end, static_cast<int>(own.w));
     const double u0 = __shfl_sync(0xffffffffu, w0, sg.first), u1 = __shfl_sync(0xffffffffu, w1, sg.first),

@@ -422,11 +422,9 @@ __device__ __forceinline__ void cam_block_flush(double (&m)[46], double* dst) {
 // Camera-major block diagonal.  One warp per item (a slice of one camera's row list, the reference's transpose block
 // structure, block_sparse_matrix.cc:784-808); each lane copies ITS (gathered) row of the next 32 rows into the warp's
 // shared-memory buffer with cp.async while the warp computes on the previous 32; the 45 packed entries stay in registers per
-// lane and are reduced across the lanes when the item ends.  Measured on Ladybug-1723 (profiles/r02_*): 42 us, i.e. the
-// 117 MB it reads arrive at 2.9 TB/s -- the kernel is bound by the DRAM access pattern of 144-byte gathers, not by latency:
-// three other organisations were built and measured and lost (register-only 43 us; one continuous cp.async stream across
-// items with three buffers 48 us; CTA-local streaming of the rows with the regrouping by camera done in shared memory by
-// quarter-warps 64 us, FP64-issue-bound at 8 warps) and are not in the build.
+// lane and are reduced across the lanes when the item ends.  The kernel is bound by the DRAM access pattern of 144-byte
+// gathers, not by latency; register-only, one continuous cp.async stream across items, and CTA-local streaming with the
+// regrouping by camera done in shared memory (FP64-issue-bound) were slower and are not in the build.
 template <bool kSchur>
 __global__ void __launch_bounds__(kCamBlkThreads, 3)
     cam_blocks_v2_kernel(ProblemView p, int num_items, const CamItem* __restrict__ items, const int* __restrict__ cam_rows,

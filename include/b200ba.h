@@ -1,4 +1,4 @@
-/* b200ba.h — C ABI of libb200ba.so: the B200-native (sm_100a) implementation of Ceres Solver's
+/* b200ba.h — C ABI of libb200ba.so: the H100-native (sm_90a) implementation of Ceres Solver's
  * Levenberg–Marquardt inner-loop hot path for bundle-adjustment-shaped problems
  * (row block 2, eliminated "e" blocks of size 3 = points, "f" blocks of size 9 = cameras).
  *

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) CUDA device (select with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -50,21 +50,23 @@ def rel_err(a, b):
     return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-300))
 
 
-def compare_lm_traces(recs, recs_o, recs_o2, keys=("cost", "step_norm", "gradient_max_norm", "tr_radius")):
+def compare_lm_traces(recs, recs_o, *recs_alt, keys=("cost", "step_norm", "gradient_max_norm", "tr_radius")):
     """GPU trace against the oracle's, with the oracle's OWN sensitivity as the yardstick.
 
-    recs_o / recs_o2: the same oracle solve with two thread counts (two summation orders of its products).  The inexact
+    recs_o / recs_alt: the same oracle solve with different thread counts (different summation orders of its products); the
+    spread of a value is its largest deviation over recs_alt.  The inexact
     Schur solve stops on a threshold after k CG iterations; while k is small the trajectory is reproducible to 1e-10 and
     north_star's 1e-6 is asserted.  Once a solve runs for 50+ iterations on the ill-conditioned reduced system, last-bit
     differences are amplified to the 1e-5 level in the step (measured: 2e-5 between oracle thread counts at 117 iterations
     on ladybug-1723) and the stopping test may fire one iteration earlier or later; from there on the tolerance is
     max(10 x oracle spread, 1e-4 -- 2e-3 after a 100+-iteration solve), a difference of up to max(2, 5 %) in the CG count is accepted (with 1e-2 on that iteration), and the
     comparison ends where the trajectories fork (different counts or accept/reject decisions)."""
-    assert len(recs) == len(recs_o) == len(recs_o2)
+    assert recs_alt and all(len(recs) == len(recs_o) == len(r) for r in recs_alt)
     loose = 0.0     # sticky: the state after a long solve carries its deviation into every later iteration
-    for a, b, b2 in zip(recs, recs_o, recs_o2):
-        ko, ko2, kg = int(b["ls_iterations"]), int(b2["ls_iterations"]), int(a["ls_iterations"])
-        if ko != ko2 or int(b["step_is_successful"]) != int(b2["step_is_successful"]):
+    for i, (a, b) in enumerate(zip(recs, recs_o)):
+        alts = [r[i] for r in recs_alt]
+        ko, kg = int(b["ls_iterations"]), int(a["ls_iterations"])
+        if any(int(b2["ls_iterations"]) != ko or int(b2["step_is_successful"]) != int(b["step_is_successful"]) for b2 in alts):
             return   # the oracle forks against itself here
         long_solve = ko >= 50
         # 50-99 CG iterations: 1e-4; 100+ (observed on the I2-recipe problem: a 143-iteration solve that ends in a REJECTED
@@ -75,7 +77,7 @@ def compare_lm_traces(recs, recs_o, recs_o2, keys=("cost", "step_norm", "gradien
         assert a["step_is_successful"] == int(b["step_is_successful"]), (a, b)
         for key in keys:
             ref = float(b[key])
-            spread = abs(float(b2[key]) - ref) / max(abs(ref), 1e-300)
+            spread = max(abs(float(b2[key]) - ref) for b2 in alts) / max(abs(ref), 1e-300)
             tol = max(1e-6, 10.0 * spread, loose)
             if kg != ko:
                 tol = max(tol, 1e-2)   # one CG iteration more or less on a 50+-iteration solve: a percent-level change of the step

@@ -2,9 +2,11 @@
 Ceres header includes Eigen, which this image does not have).  tests/mock_ceres restates the handful of Ceres-internal
 interfaces the adapter is written against; here the adapter is COMPILED (-Wall -Wextra -Werror) and LINKED against it and
 libb200ba.so, its host-side logic (problem recognition, refusal messages, Huber scale recovery, the factory predicate) is
-run on the CPU, and -- when the reference tree is present -- every restated signature is looked up in the reference
-headers.  The `-m gpu` part runs the driver's `solve` case on the device -- Create -> Evaluate -> Solve through the adapter
+run on the CPU, and every restated signature is checked against the digests of the ceres-solver headers it was
+found in (tests/golden/ceres_reference_digests.json).  The `-m gpu` part runs the driver's `solve` case on the device -- Create -> Evaluate -> Solve through the adapter
 classes -- and compares it with the oracle."""
+import hashlib
+import json
 import os
 import re
 import shutil
@@ -14,7 +16,6 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
 
 pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="needs g++")
 
@@ -103,7 +104,7 @@ def test_valid_program_reaches_the_library_and_fails_loudly_without_a_gpu(driver
 def test_adapter_classes_match_oracle(driver, tmp_path, oracle, huber):
     """Create -> CreateJacobian -> Evaluate (with and without apply_loss_function) -> SquaredColumnNorm ->
     B200IterativeSchurSolver::Solve -> RightMultiplyAndAccumulate -> ModelCostChange -> Plus through the adapter classes,
-    against the oracle (profiles/r02_adapter_mock_gpu.log)."""
+    against the oracle."""
     from ceres_solver_b200 import bal as B
     bal = B.synthetic_bal(64, 4000, 18000, seed=3)
     rp = B.ReducedProgram(bal)
@@ -141,7 +142,7 @@ def test_adapter_classes_match_oracle(driver, tmp_path, oracle, huber):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the mock against the reference tree
+# the mock against the ceres-solver headers
 
 def _norm(text):
     text = re.sub(r"//[^\n]*", " ", text)
@@ -207,14 +208,16 @@ SIGNATURES = {
 }
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "internal", "ceres")), reason="needs the reference tree")
 @pytest.mark.parametrize("rel", sorted(SIGNATURES))
 def test_mock_signatures_exist_in_the_reference(rel):
-    """Every declaration the mock restates (and the adapter relies on) is present, token for token, in the reference
-    header it cites -- `final` / `override` / export macros aside (the patch removes the `final`s, test_adapter_patch.py)."""
-    text = _norm(open(os.path.join(REF, rel)).read())
+    """Every declaration the mock restates (and the adapter relies on) is present, token for token, in the ceres-solver
+    header it cites -- `final` / `override` / export macros aside (the patch removes the `final`s, test_adapter_patch.py).
+    tools/make_reference_digests.py looked each one up in the ceres-solver tree and stored the SHA-256 of the normalised
+    declarations it found; a declaration added or changed here has to be looked up again the same way."""
+    with open(os.path.join(ROOT, "tests", "golden", "ceres_reference_digests.json")) as f:
+        found = set(json.load(f)["signatures"][rel])
     for sig in SIGNATURES[rel]:
-        assert _norm(sig) in text, (rel, sig)
+        assert hashlib.sha256(_norm(sig).encode()).hexdigest() in found, (rel, sig)
 
 
 @pytest.mark.parametrize("rel", sorted(SIGNATURES))

@@ -81,13 +81,14 @@ def test_components_match_oracle(case, oracle):
 
 @pytest.fixture(scope="module")
 def oracle_traces(case):
-    """The oracle's first three LM iterations, twice: with all host threads and with 7 -- a different summation order in
+    """The oracle's first three LM iterations with all host threads and with 7, 5 and 3 -- different summation orders in
     its own products.  The inexact solver amplifies last-bit differences once it runs for 100+ CG iterations on an
     ill-conditioned reduced system: on ladybug-1723 the oracle's step norm at LM iteration 3 (117 CG iterations) moves by
-    2e-5 between thread counts while iterations 1-2 (4 and 34 CG iterations) agree to 1e-10.  The spread between the two
-    oracle runs is therefore the resolution of the comparison."""
+    2e-5 between thread counts while iterations 1-2 (4 and 34 CG iterations) agree to 1e-10, and its |g|_inf there spans
+    5e-3 over 1, 2, 3, 5, 7 and 16 threads although some pairs agree to 2e-4.  The spread over several oracle runs is
+    therefore the resolution of the comparison."""
     out = []
-    for nt in (case.nt, 7 if case.nt != 7 else 5):
+    for nt in dict.fromkeys((case.nt, 7, 5, 3)):
         o = case.orc.default_options()
         o.num_threads = nt
         o.max_num_iterations = 3
@@ -103,7 +104,6 @@ def test_first_lm_iterations_match_oracle(case, oracle_traces, host_boundary):
     cannot reproduce its own numbers to 1e-6 under a change of summation order, measured against the oracle's own spread
     (tests/conftest.py: compare_lm_traces)."""
     from tests.conftest import compare_lm_traces
-    recs_o, recs_o2 = oracle_traces
     _, recs = case.gpu.lm_solve(case.state, case.gpu.lm_options(max_num_iterations=3), host_boundary=host_boundary)
     assert len(recs) == 4
-    compare_lm_traces(recs, recs_o, recs_o2)
+    compare_lm_traces(recs, *oracle_traces)

@@ -2,7 +2,7 @@
 
 Tolerances: north_star asks for 1e-6 relative on residuals and step norm; the component checks below are far
 tighter (FP64 everywhere, only summation order differs), the 1e-6 bound is asserted on the LM trajectories.
-Every test here needs a B200 (`-m gpu`).
+Every test here needs an H100 (`-m gpu`).
 """
 import numpy as np
 import pytest

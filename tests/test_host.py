@@ -236,15 +236,15 @@ def test_internal_point_order_plan():
 
     for bal, expect_identity in ((B.synthetic_sequence(300, 9000, 40000, seed=3), True), (B.synthetic("tiny"), None)):
         rp = B.ReducedProgram(bal)
-        perm, metrics, choice = cs.plan_point_order(rp.C, rp.P, rp.row_cam, rp.row_pt, 148)
+        perm, metrics, choice = cs.plan_point_order(rp.C, rp.P, rp.row_cam, rp.row_pt, 132)
         assert sorted(perm.tolist()) == list(range(rp.P))
         if expect_identity:
             assert choice == 0 and np.array_equal(perm, np.arange(rp.P))
-        assert metrics[0] == score(rp.row_cam.astype(np.int64), rp.row_pt.astype(np.int64), rp.P, rp.C, np.arange(rp.P), 148)
+        assert metrics[0] == score(rp.row_cam.astype(np.int64), rp.row_pt.astype(np.int64), rp.P, rp.C, np.arange(rp.P), 132)
     bal = B.synthetic_bal(400, 12000, 52000, seed=11)   # points in random order
     rp = B.ReducedProgram(bal)
-    perm, metrics, choice = cs.plan_point_order(rp.C, rp.P, rp.row_cam, rp.row_pt, 148)
+    perm, metrics, choice = cs.plan_point_order(rp.C, rp.P, rp.row_cam, rp.row_pt, 132)
     assert choice != 0 and sorted(perm.tolist()) == list(range(rp.P))
     assert metrics[choice] * 2 < metrics[0]
-    assert metrics[choice] == score(rp.row_cam.astype(np.int64), rp.row_pt.astype(np.int64), rp.P, rp.C, perm.astype(np.int64), 148)
+    assert metrics[choice] == score(rp.row_cam.astype(np.int64), rp.row_pt.astype(np.int64), rp.P, rp.C, perm.astype(np.int64), 132)
     assert metrics[choice] == min(metrics[1:])
