@@ -45,6 +45,9 @@ namespace {
 
 thread_local std::string g_error;
 constexpr int kHostThreads = 8;   // host-side vector passes of the host-boundary LM loop (the reference uses its thread pool)
+// Share of the L2 the S*x residency plan may fill (b200_create).  On an H100 (50 MB L2) the product got faster up to
+// ~24 MB resident and slower again from 32 MB on (DESIGN §3.2).
+constexpr double kL2ResidentShare = 0.5;
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.
@@ -1925,22 +1928,44 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     }
   }
 
-  if (const char* e = dev_env("B200_L2_PERSIST_MB")) {
-    // experiment: keep part of the F cells resident in L2 across the products of a PCG (persisting access window)
-    const size_t want = static_cast<size_t>(atoi(e)) << 20;
-    const size_t lim = std::min<size_t>(want, prop.persistingL2CacheMaxSize);
-    CU(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, lim));
-    cudaStreamAttrValue attr{};
-    const size_t fbytes = sizeof(double) * 18 * n;
-    const size_t win = std::min<size_t>(fbytes, prop.accessPolicyMaxWindowSize);
-    attr.accessPolicyWindow.base_ptr = h->d_values + 6 * n;
-    attr.accessPolicyWindow.num_bytes = win;
-    attr.accessPolicyWindow.hitRatio = static_cast<float>(std::min(1.0, static_cast<double>(lim) / static_cast<double>(win)));
-    attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    CU(cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &attr));
-    fprintf(stderr, "[b200ba] L2 persist: limit %zu MB (max %d MB), window %zu MB (max %d MB), hit ratio %.2f\n", lim >> 20,
-            prop.persistingL2CacheMaxSize >> 20, win >> 20, prop.accessPolicyMaxWindowSize >> 20, attr.accessPolicyWindow.hitRatio);
+  if (h->mul_v4) {
+    // L2 residency plan of S*x.  J does not change during a PCG, and every product streams the same bytes (F, E,
+    // (E'E+D^2)^-1 blocks, descriptors: 141 MB on Ladybug-1723); under the default policy a stream larger than L2 leaves
+    // nothing behind for the next product.  So a fixed share of the tiles, spread evenly through every CTA's tile range
+    // (HBM keeps streaming while the resident tiles are read from L2), is copied with evict_normal and the rest with
+    // evict_first: the resident share then survives from one product to the next.  The budget is kL2ResidentShare of the
+    // L2 minus the working set of the CG loop, which is read with the default policy; a stream within the budget is all
+    // resident.  Whole tiles: the four copies of a tile share one policy.
+    int l2_bytes = 0;
+    CU(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, h->device));
+    double stream_bytes = 0.0;
+    for (int b = 0; b < num_ctas_v2; ++b) {
+      for (int t = cta_part[b].x; t < cta_part[b].y; ++t) stream_bytes += 192.0 * wtiles[t].row_count + 48.0 * wtiles[t].pt_count + 4 * kV4MetaWords;
+      for (int t = cta_big[b].x; t < cta_big[b].y; ++t) stream_bytes += 192.0 * big_tiles[t].obs_count;
+    }
+    const double working_set = 8.0 * (8 * 9 + 81) * C                                  // rhs x r z p q seed D_f, minv
+                               + (h->world > 1 ? 2.0 * h->world * 16 * 9 * C : 0.0);    // peer exchange slots
+    double budget = std::max(0.0, kL2ResidentShare * l2_bytes - working_set);
+    const char* dev_mb = dev_env("B200_L2_RESIDENT_MB");   // 0: no plan, every copy with the default policy
+    if (dev_mb != nullptr) budget = atof(dev_mb) * (1 << 20);
+    if (const char* e = dev_env("B200_L2_RESIDENT_POLICY")) h->v2_mul.l2_last = strcmp(e, "last") == 0 ? 1 : 0;
+    const bool no_plan = dev_mb != nullptr && budget <= 0.0;
+    h->v2_mul.l2_stream = (budget >= stream_bytes || no_plan) ? 0u : static_cast<uint32_t>(std::ceil(65536.0 * (1.0 - budget / stream_bytes)));
+    if (getenv("B200_VERBOSE") != nullptr) {
+      // what the plan marks, counted the way the kernel decides it
+      const uint64_t s = h->v2_mul.l2_stream;
+      auto streamed = [&](int i) { return ((static_cast<uint64_t>(i) + 1) * s >> 16) != (static_cast<uint64_t>(i) * s >> 16); };
+      double res = 0.0;
+      for (int b = 0; b < num_ctas_v2; ++b) {
+        for (int t = cta_part[b].x; t < cta_part[b].y; ++t)
+          if (!streamed(t - cta_part[b].x)) res += 192.0 * wtiles[t].row_count + 48.0 * wtiles[t].pt_count + 4 * kV4MetaWords;
+        for (int t = cta_big[b].x; t < cta_big[b].y; ++t)
+          if (!streamed(t - cta_big[b].x)) res += 192.0 * big_tiles[t].obs_count;
+      }
+      fprintf(stderr, "[b200ba] S*x L2 plan (L2 %d MiB, budget %.1f MiB): resident %.1f MiB, streamed %.1f MiB, stride %.2f tiles (%s)\n",
+              l2_bytes >> 20, budget / (1 << 20), res / (1 << 20), (stream_bytes - res) / (1 << 20), s < 65536 ? 65536.0 / (65536 - s) : 0.0,
+              h->v2_mul.l2_last ? "evict_last" : "evict_normal");
+    }
   }
   if (getenv("B200_VERBOSE") != nullptr)
     fprintf(stderr,

@@ -84,6 +84,31 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// L2 cache policies for the hinted bulk copy below (createpolicy: a 64-bit policy word, no memory access).
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_normal() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// bulk_g2s with an L2 eviction-priority hint for the lines it brings into L2.  The hint only decides which lines L2 gives
+// up first; the bytes copied are the same.
+__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
 // TMA 1-D bulk copy shared -> global (bulk async-group completion).
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)),

@@ -42,7 +42,21 @@ struct V2View {
   int direct;                // 1: CTAs RED their (narrow) camera range straight into the output vector; 0: partials
   int per_warp_bytes;
   int variant;               // development builds only (-DB200_DEV_KNOBS): selects kernel variants for A/B runs; 0 in the product
+  // L2 residency plan of S*x (b200_create), the same for every CTA: a fraction l2_stream / 65536 of its tiles, spread
+  // evenly over its tile range, is copied with evict_first; the rest with evict_normal (evict_last if l2_last, development
+  // builds), so that it stays in L2 from one product of a PCG to the next.  0: every copy evict_normal, the default policy.
+  uint32_t l2_stream;
+  int l2_last;
 };
+
+// L2 policy of the bulk copies of entry i of a CTA's tile range under the residency plan: entry i is streamed when
+// floor((i + 1) s) != floor(i s) with s = l2_stream / 65536.  Created per copy instead of once per thread:
+// schur_mul_v4_kernel sits at the 128-register limit of 16 warps per SM.
+__device__ __forceinline__ uint64_t v4_l2_policy(const V2View& v, int i) {
+  const uint64_t s = v.l2_stream, k = static_cast<uint64_t>(i);
+  if (((k + 1) * s >> 16) != (k * s >> 16)) return l2_policy_evict_first();
+  return v.l2_last ? l2_policy_evict_last() : l2_policy_evict_normal();
+}
 
 // Row word accessors.  A CTA addresses its cameras by their position in its own camera list (direct mode: the list is
 // short, the private camera vectors live in shared memory and are flushed with REDs), or by the offset inside its camera
@@ -223,12 +237,13 @@ __device__ __forceinline__ void schur_mul_big_points_impl(const V2View& v, const
   for (int b = br.x; b < br.y; ++b) {
     const TileDesc d = v.big_tiles[b];
     if (tid == 0) {
+      const uint64_t pol = v4_l2_policy(v, b - br.x);
       mbar_arrive_expect_tx(st.bar, d.obs_count * 192u);
       for (int r0 = 0, k = 0; r0 < d.obs_count; r0 += st.chunk_rows, ++k) {
         const int rows = min(st.chunk_rows, d.obs_count - r0);
         unsigned char* dst = st.base + static_cast<size_t>(k) * st.chunk_stride;
-        bulk_g2s(dst, v.p.F() + 18 * static_cast<size_t>(d.obs_begin + r0), rows * 144u, st.bar);
-        bulk_g2s(dst + st.chunk_rows * 144, v.p.E() + 6 * static_cast<size_t>(d.obs_begin + r0), rows * 48u, st.bar);
+        bulk_g2s(dst, v.p.F() + 18 * static_cast<size_t>(d.obs_begin + r0), rows * 144u, st.bar, pol);
+        bulk_g2s(dst + st.chunk_rows * 144, v.p.E() + 6 * static_cast<size_t>(d.obs_begin + r0), rows * 48u, st.bar, pol);
       }
     }
     const bool active = tid < d.obs_count;
@@ -483,13 +498,15 @@ __host__ __device__ inline int v4_extra_offset(int stages) { return v4_bars_offs
 __host__ __device__ inline int v4_per_warp_bytes(int stages) { return v4_extra_offset(stages) + 16; }
 __host__ __device__ inline size_t v4_sx_bytes(int max_cam_span, int stage_x) { return stage_x ? v2_sy_stride(max_cam_span) * 8 : 0; }
 
+// `part_begin`: first tile of the CTA's range (the residency plan is indexed by the position of the tile inside it).
 __device__ __forceinline__ void v4_issue(const V2View& v, const double* ete_inv, unsigned char* stage, uint64_t* bar, int tile,
-                                         int row_begin, int pt_begin, int row_count, int pt_count) {
+                                         int row_begin, int pt_begin, int row_count, int pt_count, int part_begin) {
+  const uint64_t pol = v4_l2_policy(v, tile - part_begin);
   mbar_arrive_expect_tx(bar, row_count * 192u + pt_count * 48u + kV4MetaWords * 4u);
-  bulk_g2s(stage, v.p.F() + 18 * static_cast<size_t>(row_begin), row_count * 144u, bar);
-  bulk_g2s(stage + 4608, v.p.E() + 6 * static_cast<size_t>(row_begin), row_count * 48u, bar);
-  bulk_g2s(stage + 6144, ete_inv + 6 * static_cast<size_t>(pt_begin), pt_count * 48u, bar);
-  bulk_g2s(stage + 7680, v.tile_meta + static_cast<size_t>(kV4MetaWords) * tile, kV4MetaWords * 4u, bar);
+  bulk_g2s(stage, v.p.F() + 18 * static_cast<size_t>(row_begin), row_count * 144u, bar, pol);
+  bulk_g2s(stage + 4608, v.p.E() + 6 * static_cast<size_t>(row_begin), row_count * 48u, bar, pol);
+  bulk_g2s(stage + 6144, ete_inv + 6 * static_cast<size_t>(pt_begin), pt_count * 48u, bar, pol);
+  bulk_g2s(stage + 7680, v.tile_meta + static_cast<size_t>(kV4MetaWords) * tile, kV4MetaWords * 4u, bar, pol);
 }
 
 // Adds one 9-vector per row into replica `sy_rep` that only THIS warp touches: after the same warp-level
@@ -578,7 +595,7 @@ __device__ __forceinline__ void v4_prime(const V2View& v, const double* ete_inv,
     int t = c.part.x + (threadIdx.x >> 5);
     for (int s = 0; s < v.stages && t < c.part.y; ++s, t += v.warps) {
       const WarpTile wt = v.wtiles[t];
-      v4_issue(v, ete_inv, c.wbase() + s * kV4StageBytes, c.bars() + s, t, wt.row_begin, wt.pt_begin, wt.row_count, wt.pt_count);
+      v4_issue(v, ete_inv, c.wbase() + s * kV4StageBytes, c.bars() + s, t, wt.row_begin, wt.pt_begin, wt.row_count, wt.pt_count, c.part.x);
     }
   }
 }
@@ -661,7 +678,7 @@ __device__ __forceinline__ void v4_tiles(const V2View& v, const double* ete_inv,
     __syncwarp();  // every lane is done with the ring slot (and with the previous tile's scratch)
     if (lane == 0 && (nxt.z & 0xffffu) != 0u)
       v4_issue(v, ete_inv, stage, c.bars() + s, tile + reissue, static_cast<int>(nxt.x), static_cast<int>(nxt.y),
-               static_cast<int>(nxt.z & 0xffffu), static_cast<int>(nxt.z >> 16));
+               static_cast<int>(nxt.z & 0xffffu), static_cast<int>(nxt.z >> 16), part.x);
     double t0 = 0.0, t1 = 0.0, w0 = 0.0, w1 = 0.0, w2 = 0.0;
     if (active) {
       double xc[9];
