@@ -18,6 +18,7 @@ _ip = C.POINTER(C.c_int32)
 
 OK = 0
 ERR_EVALUATION_FAILED = -3
+ERR_UNSUPPORTED = -6
 LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR = 0, 1, 2, 3
 PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION = 0, 1, 2, 3
 ITERATIVE_SCHUR, DENSE_SCHUR = 0, 1

@@ -1968,11 +1968,13 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     }
   }
   if (getenv("B200_VERBOSE") != nullptr)
+    // mul: the S*x family (tile = the CTA-tile kernels everywhere); diag: the block-diagonal pass precond_update_dev runs
     fprintf(stderr,
-            "[b200ba] C=%d P=%d N=%d wtiles=%zu big(+slices)=%zu huge=%d span=%d direct=%d v2(w=%d,s=%d,r=%d) mul(%s w=%d,s=%d,r=%d,smem=%zu) folded=%d v2b=%d cam_major=%d\n",
+            "[b200ba] C=%d P=%d N=%d wtiles=%zu big(+slices)=%zu huge=%d span=%d direct=%d v2(w=%d,s=%d,r=%d) mul(%s w=%d,s=%d,r=%d,smem=%zu) folded=%d v2b=%d cam_major=%d diag=%s\n",
             C, P, N, wtiles.size(), big_tiles.size(), h->num_huge, max_cam_span, h->v2.direct, h->v2.warps, h->v2.stages, h->v2.replicas,
-            h->mul_v4 ? (h->mul_v4_owned ? "v4-owned" : "v4") : (h->mul_v3 ? "v3" : "v2"), h->v2_mul.warps, h->v2_mul.stages, h->v2_mul.replicas, h->mul_smem,
-            h->big_folded ? 1 : 0, h->v2b_ok ? 1 : 0, h->cam_major_ok ? 1 : 0);
+            !h->v2_ok ? "tile" : h->mul_v4 ? (h->mul_v4_owned ? "v4-owned" : "v4") : "v3", h->v2_mul.warps, h->v2_mul.stages, h->v2_mul.replicas, h->mul_smem,
+            h->big_folded ? 1 : 0, h->v2b_ok ? 1 : 0, h->cam_major_ok ? 1 : 0,
+            h->cam_major_ok ? "cam_major" : (h->v2b_ok && h->diag_v2_replicas > 0) ? "v2" : "tile");
   for (int k = 0; k < K_COUNT; ++k) h->grid_tile[k] = std::max(1, std::min(h->num_tiles, h->sm_count * 4));
   h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<true>, tile_smem_bytes<3, 1>());
   h->grid_tile[K_EVAL_COST] = tile_grid(h, evaluate_kernel<false>, tile_smem_bytes<3, 1>());

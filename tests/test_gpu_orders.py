@@ -1,23 +1,22 @@
 """The library keeps its own point order and per-CTA camera lists (b200_create); what crosses the ABI stays in the
-caller's order.  Three structures exercise the three code paths, each against the oracle through every entry point:
+caller's order.  Three structures exercise the three orders, each against the oracle through every entry point
+(tests/entry_points.py):
 
   circle   SURVEY 8d I2 recipe (cameras on a circle, each point seen by cameras spread over a window around its
            azimuth), points in RANDOM order  -> internal re-ordering + boundary permutations + camera lists with
            wrap-around at camera 0 / C-1
-  scatter  every point sees cameras drawn uniformly from all of them: no order has locality -> the id-range / partial
-           vector kernels (schur_mul_v3, jtj_v2, CTA-tile evaluate / init) and cam_reduce_kernel
+  scatter  every point sees cameras drawn uniformly from all 3000 of them: no order has locality.  Its per-CTA camera
+           span is all 3000 cameras, and one camera vector of that size does not fit in shared memory next to the tile
+           buffers, so every operation runs on the CTA-tile kernels.  The id-range kernels (schur_mul_v3, jtj_v2,
+           cam_reduce_kernel) are tested on their own fixture in tests/test_gpu_dispatch.py.
   sorted   the circle problem with the points already sorted by azimuth -> the caller's order is kept (identity)
 """
 import numpy as np
 import pytest
 
+from tests.entry_points import Case, check_every_entry_point, check_lm_trajectory, oracle_lm_traces
+
 pytestmark = pytest.mark.gpu
-
-
-def relerr(a, b):
-    a = np.asarray(a, dtype=float)
-    b = np.asarray(b, dtype=float)
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-300))
 
 
 def _scatter_problem(C=3000, P=35000, N=150000, seed=5):
@@ -57,100 +56,22 @@ def cs():
     return m
 
 
-class Case:
-    def __init__(self, cs, oracle, bal):
-        from ceres_solver_b200 import bal as B
-        self.rp = B.ReducedProgram(bal)
-        self.orc = oracle.BaProgram(bal.C, bal.P, bal.cam_idx, bal.pt_idx, np.ascontiguousarray(bal.obs).ravel())
-        self.gpu = cs.Problem(self.rp.C, self.rp.P, self.rp.row_cam, self.rp.row_pt, self.rp.row_obs)
-        self.state = self.rp.state(bal)
-
-
 @pytest.fixture(scope="module", params=["circle", "scatter", "sorted"])
 def case(request, cs, oracle):
     c = Case(cs, oracle, _make(request.param))
     yield c
-    c.gpu.close()
+    c.close()
 
 
 def test_every_entry_point_in_caller_order(case, oracle):
-    gpu, orc = case.gpu, case.orc
-    ok, cost, res, grad = gpu.evaluate(case.state)
-    ok_o, cost_o, res_o, grad_o = orc.evaluate(case.state, nt=8)
-    assert ok and ok_o and abs(cost - cost_o) <= 1e-12 * cost_o
-    assert relerr(res, res_o) < 1e-12 and relerr(grad, grad_o) < 1e-10
-    J = orc.jacobian()
-    v = gpu.jacobian_values()
-    assert relerr(v, J.values()) < 1e-12
-    rng = np.random.RandomState(3)
-    x = rng.randn(gpu.num_parameters)
-    y = rng.randn(gpu.num_residuals)
-    assert relerr(gpu.squared_column_norm(), J.squared_column_norm()) < 1e-12
-    assert relerr(gpu.right_multiply(x), J.right_multiply(x)) < 1e-12
-    assert relerr(gpu.left_multiply(y), J.left_multiply(y)) < 1e-11
-    # PartitionedMatrixView single products (E x, F x, E'y, F'y), accumulate semantics
-    xe, xf = rng.randn(3 * gpu.P), rng.randn(9 * gpu.C)
-    y0 = rng.randn(gpu.num_residuals)
-    nr = gpu.num_residuals
-    assert relerr(gpu.partitioned_multiply(0, xe, y0), y0 + J.pmv(gpu.P, 0, xe, nr, nt=8)) < 1e-12
-    assert relerr(gpu.partitioned_multiply(1, xf, y0), y0 + J.pmv(gpu.P, 1, xf, nr, nt=8)) < 1e-12
-    assert relerr(gpu.partitioned_multiply(2, y, xe), xe + J.pmv(gpu.P, 2, y, 3 * gpu.P, nt=8)) < 1e-12
-    assert relerr(gpu.partitioned_multiply(3, y, xf), xf + J.pmv(gpu.P, 3, y, 9 * gpu.C, nt=8)) < 1e-11
-    # set_values round trip (in the caller's layout)
-    gpu.set_jacobian_values(2.0 * v)
-    assert relerr(gpu.right_multiply(x), 2.0 * J.right_multiply(x)) < 1e-12
-    gpu.set_jacobian_values(v)
-    s = 1.0 / (1.0 + np.sqrt(J.squared_column_norm()))
-    gpu.scale_columns(s)
-    J.scale_columns(s, nt=8)
-    assert relerr(gpu.jacobian_values(), J.values()) < 1e-14
-    D = np.sqrt(np.clip(J.squared_column_norm(), 1e-6, 1e32) / 1e4)
-    expect = J.left_multiply(J.right_multiply(x, nt=8), nt=8) + D * D * x
-    assert relerr(gpu.jtj_multiply(x, D), expect) < 1e-11
-    assert relerr(gpu.jtj_multiply(x, None), J.left_multiply(J.right_multiply(x, nt=8), nt=8)) < 1e-11
-    isc = oracle.ImplicitSchur(J, gpu.P, want_ftf=False, nt=8)
-    isc.init(D, res_o)
-    gpu.schur_init(res, D)
-    assert relerr(gpu.schur_rhs(), isc.rhs()) < 1e-9
-    assert relerr(gpu.schur_ete_inverse(), isc.ete_inverse()) < 1e-9
-    u = rng.randn(9 * gpu.C)
-    assert relerr(gpu.schur_multiply(u), isc.right_multiply(u)) < 1e-9
-    assert relerr(gpu.schur_back_substitute(u), isc.back_substitute(u)) < 1e-9
-    C = gpu.C
-    diag, _ = J.schur_eliminate(gpu.P, None, D, diagonal_only=True, diag_len=81 * C, nt=8, n_f=9 * C)
-    blocks, _ = gpu.schur_jacobi_update()
-    assert relerr(blocks, diag) < 1e-9
-    step = rng.randn(gpu.num_parameters) * 1e-3
-    Js = J.right_multiply(step, nt=8)
-    assert abs(gpu.model_cost_change(step) - (-Js @ (res_o + 0.5 * Js))) <= 1e-9 * abs(Js @ res_o)
-    # linear solves
-    xs, its, term = gpu.schur_solve(res, D, gpu.solver_options(q_tolerance=1e-3, r_tolerance=-1.0))
-    xo, its_o, term_o = J.linear_solve(gpu.P, res_o, D, solver=0, q_tolerance=1e-3, r_tolerance=-1.0, nt=8)
-    assert (its, term) == (its_o, term_o)
-    assert relerr(xs, xo) < 1e-7
-    if 9 * C <= 4000:   # the explicit reduced system is dense: small camera counts only
-        xd, _, td = gpu.dense_schur_solve(res, D)
-        xdo, _, tdo = J.linear_solve(gpu.P, res_o, D, solver=1, nt=8)
-        assert td == tdo and relerr(xd, xdo) < 1e-7
+    check_every_entry_point(case, oracle)
 
 
 @pytest.fixture(scope="module")
 def oracle_traces(case):
-    """Four LM iterations of the oracle with two thread counts: the spread between them is what a change of summation order
-    does to the inexact trajectory (tests/test_gpu_headline.py explains), i.e. the resolution of the comparison."""
-    out = []
-    for nt in (8, 3):
-        o = case.orc.default_options()
-        o.num_threads = nt
-        o.max_num_iterations = 4
-        state_o, recs_o, _ = case.orc.solve(case.state, o)
-        out.append((state_o, recs_o))
-    return out
+    return oracle_lm_traces(case, 4)
 
 
 @pytest.mark.parametrize("host_boundary", [False, True])
 def test_lm_trajectory(case, oracle_traces, host_boundary):
-    from tests.conftest import compare_lm_traces
-    (state_o, recs_o), (state_o2, recs_o2) = oracle_traces
-    state, recs = case.gpu.lm_solve(case.state, case.gpu.lm_options(max_num_iterations=4), host_boundary=host_boundary)
-    compare_lm_traces(recs, recs_o, recs_o2, keys=("cost", "step_norm"))
+    check_lm_trajectory(case, oracle_traces, 4, host_boundary)

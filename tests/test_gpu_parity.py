@@ -314,10 +314,9 @@ def test_lm_trajectory_tiny(host_boundary, tiny_case):
     _compare_traces(recs[:4], recs_o[:4])  # later iterations sit at the noise floor of the CG stopping rule
 
 
-def test_ragged_structure_and_duplicates(cs, oracle):
+def ragged_bal():
     """Degree-1 points, a point seen twice by the same camera (chunk buffer accumulation,
     schur_eliminator_impl.h:493-507), cameras with very different loads, tiles with many tiny points."""
-    rng = np.random.RandomState(5)
     from ceres_solver_b200 import bal as B
     base = B.synthetic_bal(8, 400, 1200, seed=7, max_degree=8)
     cam = base.cam_idx.copy()
@@ -333,8 +332,12 @@ def test_ragged_structure_and_duplicates(cs, oracle):
     for p in range(10, 20):
         idx = np.flatnonzero(pt == p)
         keep[idx[1:]] = False
-    bal = B.Bal(cam[keep], pt[keep], obs[keep], base.cameras, base.points)
-    case = Case(cs, oracle, bal)
+    return B.Bal(cam[keep], pt[keep], obs[keep], base.cameras, base.points)
+
+
+def test_ragged_structure_and_duplicates(cs, oracle):
+    rng = np.random.RandomState(5)
+    case = Case(cs, oracle, ragged_bal())
     J, b, D = _scaled_system(case)
     isc = oracle.ImplicitSchur(J, case.gpu.P, nt=1)
     isc.init(D, b)
