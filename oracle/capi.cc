@@ -365,7 +365,8 @@ void* orc_ba_jacobian(void* h) { return &static_cast<BaProgram*>(h)->jacobian; }
 
 struct orc_solve_options {
   int linear_solver, preconditioner, max_num_iterations, max_linear_solver_iterations,
-      min_linear_solver_iterations, jacobi_scaling, num_threads, use_spse_initialization;
+      min_linear_solver_iterations, jacobi_scaling, num_threads, use_spse_initialization,
+      max_num_consecutive_invalid_steps;
   double eta, initial_trust_region_radius, max_trust_region_radius, min_trust_region_radius,
       min_relative_decrease, min_lm_diagonal, max_lm_diagonal, function_tolerance, gradient_tolerance,
       parameter_tolerance;
@@ -380,6 +381,7 @@ void orc_solve_options_default(orc_solve_options* o) {
   o->jacobi_scaling = d.jacobi_scaling;
   o->num_threads = d.num_threads;
   o->use_spse_initialization = 0;
+  o->max_num_consecutive_invalid_steps = d.max_num_consecutive_invalid_steps;
   o->eta = d.eta;
   o->initial_trust_region_radius = d.initial_trust_region_radius;
   o->max_trust_region_radius = d.max_trust_region_radius;
@@ -408,6 +410,7 @@ int orc_ba_solve(void* h, const orc_solve_options* o, double* state_inout, doubl
   so.jacobi_scaling = o->jacobi_scaling;
   so.num_threads = o->num_threads;
   so.use_spse_initialization = o->use_spse_initialization;
+  so.max_num_consecutive_invalid_steps = o->max_num_consecutive_invalid_steps;
   so.eta = o->eta;
   so.initial_trust_region_radius = o->initial_trust_region_radius;
   so.max_trust_region_radius = o->max_trust_region_radius;

@@ -294,7 +294,8 @@ class BalProblem:
 class SolveOptions(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("linear_solver", "preconditioner", "max_num_iterations",
                                        "max_linear_solver_iterations", "min_linear_solver_iterations",
-                                       "jacobi_scaling", "num_threads", "use_spse_initialization")] + \
+                                       "jacobi_scaling", "num_threads", "use_spse_initialization",
+                                       "max_num_consecutive_invalid_steps")] + \
                [(n, C.c_double) for n in ("eta", "initial_trust_region_radius", "max_trust_region_radius",
                                           "min_trust_region_radius", "min_relative_decrease", "min_lm_diagonal",
                                           "max_lm_diagonal", "function_tolerance", "gradient_tolerance",

@@ -30,13 +30,16 @@ def parse_plan(text):
 
 
 class Case:
-    """One BAL problem set up identically for the oracle and for the GPU library."""
+    """One BAL problem set up identically for the oracle and for the GPU library, with the trivial loss
+    (loss_type = LOSS_TRIVIAL) or Huber(loss_a) (LOSS_HUBER)."""
 
-    def __init__(self, cs, oracle, bal):
+    def __init__(self, cs, oracle, bal, loss_type=0, loss_a=1.0):
         from ceres_solver_b200 import bal as B
         self.rp = B.ReducedProgram(bal)
-        self.orc = oracle.BaProgram(bal.C, bal.P, bal.cam_idx, bal.pt_idx, np.ascontiguousarray(bal.obs).ravel())
-        self.gpu = cs.Problem(self.rp.C, self.rp.P, self.rp.row_cam, self.rp.row_pt, self.rp.row_obs)
+        self.orc = oracle.BaProgram(bal.C, bal.P, bal.cam_idx, bal.pt_idx, np.ascontiguousarray(bal.obs).ravel(),
+                                    use_huber=loss_type == cs.LOSS_HUBER, huber_a=loss_a)
+        self.gpu = cs.Problem(self.rp.C, self.rp.P, self.rp.row_cam, self.rp.row_pt, self.rp.row_obs, loss_type=loss_type,
+                              loss_a=loss_a)
         self.state = self.rp.state(bal)
 
     def close(self):
@@ -47,7 +50,12 @@ def _inv_blocks(flat):
     return np.linalg.inv(flat.reshape(-1, 9, 9)).ravel()
 
 
-def check_every_entry_point(case, oracle):
+def check_every_entry_point(case, oracle, shared_inputs=False):
+    """shared_inputs: once evaluate has been checked, the oracle's Jacobian and residuals are replaced by the GPU's, so
+    that every product and solve after it is compared on identical inputs.  A robust loss needs that: the weight
+    sqrt(a / |r|) of an outlier row carries the relative rounding error of its residual, a small difference of two large
+    numbers, into every entry of its Jacobian row (~1e-12 relative, measured on the fixtures of test_gpu_dispatch.py),
+    three orders of magnitude above what the products below are held to."""
     gpu, orc = case.gpu, case.orc
     ok, cost, res, grad = gpu.evaluate(case.state)
     ok_o, cost_o, res_o, grad_o = orc.evaluate(case.state, nt=8)
@@ -56,6 +64,9 @@ def check_every_entry_point(case, oracle):
     J = orc.jacobian()
     v = gpu.jacobian_values()
     assert relerr(v, J.values()) < 1e-12
+    if shared_inputs:
+        J.set_values(v)
+        res_o = res
     # cost-only evaluation: same cost, Jacobian untouched
     ok, cost2, _, _ = gpu.evaluate(case.state, want_residuals=False, want_gradient=False, want_jacobian=False)
     assert ok and abs(cost2 - cost_o) <= 1e-12 * cost_o
@@ -148,3 +159,30 @@ def check_lm_trajectory(case, traces, iterations, host_boundary, max_cg=None):
         o.linear_solver.max_num_iterations = max_cg
     _, recs = case.gpu.lm_solve(case.state, o, host_boundary=host_boundary)
     compare_lm_traces(recs, *traces, keys=("cost", "step_norm"))
+
+
+INT_FIELDS = ("iteration", "ls_iterations", "step_is_valid", "step_is_successful")
+RELATIVE_FIELDS = ("cost", "gradient_max_norm", "gradient_norm", "step_norm", "tr_radius", "model_cost_change")
+
+
+def compare_lm_traces_exact(recs, recs_o):
+    """Every field of every record of a short solve against the oracle's (the same options on both sides).  While every
+    linear solve is short, the two trajectories differ only by summation order, ~1e-10 relative, so this holds them to
+    1e-9: the iteration and CG counts and the valid / accepted decisions equal; cost, gradient norms, step norm, radius
+    and model cost change to 1e-9 relative; the cost change to 1e-9 of the cost (it is a difference of two costs); the
+    step quality rho to 1e-6 max(1, |rho|) (a quotient of two differences).  A zero on the oracle's side (the step norm
+    before the first accepted step, an invalid step's model cost change) must be an exact zero on the GPU's.
+
+    The gradient norms also get 1e-12 of the initial record's: the gradient J'r is a sum whose terms do not shrink as the
+    solve converges, so its rounding error stays at the scale of the initial gradient while the gradient itself drops by
+    orders of magnitude (measured on `tiny`: record 2's max norm, 1e4 below the initial one, moves by up to 1.6e-9
+    relative between GPU and oracle and by 4e-10 between two oracle runs with the same thread count)."""
+    assert len(recs) == len(recs_o), ([r["iteration"] for r in recs], [int(r["iteration"]) for r in recs_o])
+    for a, b in zip(recs, recs_o):
+        for key in INT_FIELDS:
+            assert int(a[key]) == int(b[key]), (key, a, b)
+        for key in RELATIVE_FIELDS:
+            floor = 1e-12 * abs(recs_o[0][key]) if key in ("gradient_max_norm", "gradient_norm") else 0.0
+            assert abs(a[key] - b[key]) <= 1e-9 * abs(b[key]) + floor, (key, a, b)
+        assert abs(a["cost_change"] - b["cost_change"]) <= 1e-9 * abs(b["cost"]), ("cost_change", a, b)
+        assert abs(a["tr_ratio"] - b["tr_ratio"]) <= 1e-6 * max(1.0, abs(b["tr_ratio"])), ("tr_ratio", a, b)

@@ -373,10 +373,9 @@ def _project(cameras, points, cam_idx, pt_idx):
     return np.stack([c[:, 6] * d * xp, c[:, 6] * d * yp], axis=1)
 
 
-@pytest.fixture(scope="module")
-def huge_case(cs, oracle):
+def huge_bal():
     """Points observed by 129, 150, 257 and all 400 cameras next to ordinary ones: more than kTile = 128 rows per point
-    (chunk tiles + huge_kernels.cuh)."""
+    (chunk tiles + huge_kernels.cuh), and points of 33 and 128 rows."""
     from ceres_solver_b200 import bal as B
     rng = np.random.RandomState(11)
     base = B.synthetic_bal(400, 600, 3000, seed=21, max_degree=40)
@@ -391,8 +390,12 @@ def huge_case(cs, oracle):
         cam.append(extra)
         pt.append(pts_i)
         obs.append(_project(base.cameras, base.points, extra, pts_i) + rng.normal(0.0, 0.5, (extra.size, 2)))
-    bal = B.Bal(np.concatenate(cam), np.concatenate(pt), np.concatenate(obs), base.cameras, base.points)
-    return Case(cs, oracle, bal)
+    return B.Bal(np.concatenate(cam), np.concatenate(pt), np.concatenate(obs), base.cameras, base.points)
+
+
+@pytest.fixture(scope="module")
+def huge_case(cs, oracle):
+    return Case(cs, oracle, huge_bal())
 
 
 def test_huge_points_components(huge_case, oracle):
