@@ -17,6 +17,7 @@ _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int32)
 
 OK = 0
+ERR_INVALID_ARGUMENT = -1
 ERR_EVALUATION_FAILED = -3
 ERR_UNSUPPORTED = -6
 LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR = 0, 1, 2, 3

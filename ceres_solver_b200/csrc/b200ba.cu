@@ -467,8 +467,11 @@ int sqnorm_dev(b200_handle* h, double* d_out);
 
 // d_sqnorm (optional): squared column norms of the Jacobian as written (after the fused scaling), for free with the
 // warp-tile kernel; the caller falls back to sqnorm_dev when *sqnorm_done comes back false.
+// J is computed (and checked) when the Jacobian or the gradient is asked for, and stored only when want_jacobian: a
+// gradient-only evaluation leaves the device-resident Jacobian as it was, as Ceres leaves it with jacobian == NULL.
 int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, double* d_gradient, bool want_jacobian,
                  const double* d_scale, double* cost_out, double* d_sqnorm = nullptr, bool* sqnorm_done = nullptr) {
+  if (!want_jacobian) d_sqnorm = nullptr;   // the column norms are those of the stored Jacobian
   EvalArgs a{};
   a.state = d_state;
   a.residuals = d_residuals;
@@ -500,13 +503,16 @@ int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, dou
     if (d_sqnorm != nullptr) CU(cudaMemsetAsync(d_sqnorm + coff, 0, sizeof(double) * 9 * h->C, h->stream));
     if (d_sqnorm != nullptr) OK(huge_zero(h, d_sqnorm));
     OK(launch(h, K_EVAL_JAC, [&] {
-      evaluate_v2_kernel<<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
+      if (want_jacobian) evaluate_v2_kernel<true><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
+      else evaluate_v2_kernel<false><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
     }));
     num_partials = h->v2.num_ctas;
     if (h->num_big_tiles > 0) {  // the few >32-row points: CTA-tile kernels on their tiles only
       a.cost_partial = h->d_tile_partial + num_partials;
       OK(launch(h, K_EVAL_JAC, [&] {
-        evaluate_kernel<true><<<std::min(h->num_big_tiles, h->sm_count * 2), kTile, smem, h->stream>>>(h->view_big, a);
+        const int grid = std::min(h->num_big_tiles, h->sm_count * 2);
+        if (want_jacobian) evaluate_kernel<true><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
+        else evaluate_kernel<true, false><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
       }, false));
       num_partials += h->num_big_tiles;
       if (d_sqnorm != nullptr)
@@ -519,7 +525,10 @@ int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, dou
       if (sqnorm_done != nullptr) *sqnorm_done = true;
     }
   } else if (with_j) {
-    OK(launch(h, K_EVAL_JAC, [&] { evaluate_kernel<true><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a); }));
+    OK(launch(h, K_EVAL_JAC, [&] {
+      if (want_jacobian) evaluate_kernel<true><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
+      else evaluate_kernel<true, false><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
+    }));
   } else {
     OK(launch(h, K_EVAL_COST, [&] { evaluate_kernel<false><<<h->grid_tile[K_EVAL_COST], kTile, smem, h->stream>>>(h->view, a); }));
   }
@@ -1919,7 +1928,8 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
       }
       if (h->diag_v2_smem > lim) h->diag_v2_replicas = 0;  // falls back to the CTA-tile kernel
       if (h->eval_v2_smem <= lim && h->init_v2_smem <= lim) {
-        CU(cudaFuncSetAttribute(evaluate_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
+        CU(cudaFuncSetAttribute(evaluate_v2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
+        CU(cudaFuncSetAttribute(evaluate_v2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
         CU(cudaFuncSetAttribute(schur_init_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
         CU(cudaFuncSetAttribute(diag_blocks_v2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
         CU(cudaFuncSetAttribute(diag_blocks_v2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(prop.sharedMemPerBlockOptin) - 1024));
@@ -2123,6 +2133,8 @@ int b200_evaluate(b200_handle* h, const double* state, double* cost, double* res
   if (h == nullptr || state == nullptr || cost == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   CU(cudaSetDevice(h->device));
   OK(up_params(h, h->d_state, state));
+  // an evaluation that asks for residuals overwrites d_residuals: they are the resident residuals again only if it succeeds
+  if (residuals != nullptr) h->residuals_resident = false;
   OK(evaluate_dev(h, h->d_state, residuals != nullptr ? h->d_residuals : nullptr,
                   gradient != nullptr ? h->d_gradient : nullptr, want_jacobian != 0, nullptr, cost));
   if (residuals != nullptr) {

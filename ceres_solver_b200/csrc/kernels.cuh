@@ -143,7 +143,9 @@ struct EvalArgs {
   double loss_a;
 };
 
-template <bool kWantJ>
+// kStoreJ = false (gradient without the Jacobian): J is computed, checked and used for the gradient, but the stored
+// Jacobian is left as it is.  A template parameter, so that the instantiation the LM loop runs is the same code.
+template <bool kWantJ, bool kStoreJ = kWantJ>
 __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const TileSmem s = carve_smem<3, 1>(smem_raw);
@@ -261,7 +263,7 @@ __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs
     if (kWantJ) {
       fence_proxy_async_smem();
       __syncthreads();
-      if (tid == 0) {
+      if (kStoreJ && tid == 0) {
         bulk_s2g(p.E() + 6 * static_cast<size_t>(d.obs_begin), s.sE, d.obs_count * 48u);
         bulk_s2g(p.F() + 18 * static_cast<size_t>(d.obs_begin), s.sF, d.obs_count * 144u);
         bulk_commit();

@@ -102,6 +102,8 @@ __host__ __device__ inline int eval_v2_per_warp_bytes() { return 32 * 144 + 32 *
 
 // Evaluate residuals, Jacobian (written through a per-warp staging buffer + TMA bulk store), cost, gradient and the
 // squared column norms of the Jacobian as written (i.e. after the fused Jacobi scaling).
+// kStoreJ = false (gradient without the Jacobian): as evaluate_kernel<true, false>, the Jacobian is left as it is.
+template <bool kStoreJ>
 __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v, EvalV2Args a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -245,6 +247,7 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
       if (owned) cam_accumulate9_owned(my_q, cam_l, active, qc);
       else cam_accumulate<9>(my_q, cam_l, active, qc);
     }
+    if (!kStoreJ) continue;
     // Jacobian cells: stage the warp's rows contiguously, then one TMA bulk store each for E and F
     if (store_pending) {
       if (lane == 0) bulk_wait_read_all();

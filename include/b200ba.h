@@ -90,8 +90,12 @@ int b200_num_parameters(const b200_handle* h);     /* Evaluator::NumParameters  
 int64_t b200_num_residuals(const b200_handle* h);  /* Evaluator::NumResiduals    evaluator.h:158 */
 
 /* ---- Evaluator (internal/ceres/evaluator.h:116-121, ProgramEvaluator::Evaluate program_evaluator.h:137-304)
- * residuals / gradient may be NULL; want_jacobian != 0 refreshes the device-resident Jacobian.
- * gradient = J'r of the unscaled Jacobian.  Returns B200_ERR_EVALUATION_FAILED where Evaluate returns false. */
+ * residuals / gradient may be NULL; want_jacobian != 0 refreshes the device-resident Jacobian, and want_jacobian == 0
+ * leaves it untouched, also when the gradient is asked for.  gradient = J'r of the unscaled Jacobian.
+ * Returns B200_ERR_EVALUATION_FAILED where Evaluate returns false (residual_block.cc:100-131, program_evaluator.h:205-292):
+ * a non-finite residual, a non-finite Jacobian entry whenever J is computed (for the Jacobian or the gradient), or a
+ * non-finite total cost.  A failed call that asked for residuals leaves no resident residuals (see b200_schur_solve);
+ * a failed call that asked for the Jacobian leaves the device-resident Jacobian undefined. */
 int b200_evaluate(b200_handle* h, const double* state, double* cost, double* residuals, double* gradient,
                   int want_jacobian);
 /* Evaluator::EvaluateOptions::apply_loss_function (evaluator.h:101-102): apply == 0 makes the following evaluations
@@ -146,7 +150,10 @@ typedef struct b200_solver_summary { /* LinearSolver::Summary, linear_solver.h:3
 void b200_solver_options_default(b200_solver_options* o);
 /* b == NULL: b is the residual vector the last b200_evaluate produced, which is still in HBM (the minimizer passes
  * exactly that vector, trust_region_minimizer.cc:399-402 via levenberg_marquardt_strategy.cc:116; the adapter
- * compares the pointer with the one it filled in Evaluate and skips the 16N-byte upload). */
+ * compares the pointer with the one it filled in Evaluate and skips the 16N-byte upload).  Only a successful
+ * b200_evaluate with residuals != NULL produces it; after one that asked for residuals and failed there is none, and
+ * b == NULL returns B200_ERR_INVALID_ARGUMENT until the next successful one (as does b200_model_cost_change).  Calls
+ * without residuals (cost only, Jacobian only) leave it as it was. */
 int b200_schur_solve(b200_handle* h, const double* b, const double* D, const b200_solver_options* opts,
                      double* x, b200_solver_summary* summary);
 
