@@ -38,6 +38,7 @@
 #include "spse_kernels.cuh"
 #include "huge_kernels.cuh"
 #include "dense_schur.cuh"
+#include "explicit_schur.cuh"
 
 using namespace b200;
 
@@ -48,6 +49,14 @@ constexpr int kHostThreads = 8;   // host-side vector passes of the host-boundar
 // Share of the L2 the S*x residency plan may fill (b200_create).  On an H100 (50 MB L2) the product got faster up to
 // ~24 MB resident and slower again from 32 MB on (DESIGN §3.2).
 constexpr double kL2ResidentShare = 0.5;
+// Explicit S (explicit_schur.cuh) when the implicit product's stream is at least kXsByteRatio times the bytes of a
+// product on the explicit upper triangle (each off-diagonal block read twice), does not fit the L2 residency budget
+// (then the implicit product is served from L2 and the assembly cannot pay for itself), and S with its row-pair list
+// fits kXsMaxBytes (the assembly time grows with the row pairs, and a solve of few CG iterations cannot repay it).
+// Measured on one H100 (DESIGN §3): Ladybug-1723 (ratio 3.3, 40 MB) is faster explicit; ladybug-1723-random (ratio 0.47),
+// C16 (stream within the L2 budget) and Venice-1778 (186 MB, 3-10 CG iterations per solve) are faster implicit.
+constexpr double kXsByteRatio = 2.0;
+constexpr double kXsMaxBytes = 128.0 * (1 << 20);
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.
@@ -295,7 +304,18 @@ struct b200_handle {
   CamItem* d_cam_items = nullptr;
   int* d_cam_rows = nullptr;
   double* d_q3 = nullptr;
-  double* d_ybig = nullptr;   // RED target of the big-point kernel inside the PCG (consumed + zeroed by cg_vector_kernel)
+  // explicit S (explicit_schur.cuh), single GPU, chosen by b200_create from the camera graph
+  bool xs = false;
+  bool xs_ready = false;        // S holds the assembly for the current implicit-Schur initialisation
+  bool xs_diag_ready = false;   // ... and d_upper45 still holds its diagonal blocks
+  int xs_grid = 0;
+  XsView xsv{};
+  int num_xs_long = 0, num_xs_short = 0;   // blocks assembled by a CTA / by a warp each
+  int *d_xs_blk_row = nullptr, *d_xs_blk_col = nullptr, *d_xs_pair_ptr = nullptr, *d_xs_list_ptr = nullptr, *d_xs_warp_cam = nullptr;
+  int* d_xs_order = nullptr;   // [long blocks | short blocks]
+  int2 *d_xs_pairs = nullptr, *d_xs_list = nullptr;
+  double* d_xs_S = nullptr;
+  double* d_ybig = nullptr;  // RED target of the big-point kernel inside the PCG (consumed + zeroed by cg_vector_kernel)
   double* d_red = nullptr;    // per-CTA partial sums of cg_vector_kernel
   // multi-GPU exchange of the per-iteration partial products over NVLink peer memory (cg_kernel.cuh: xchg_push_kernel +
   // the gather in cg_vector_kernel); replaces the ncclAllReduce inside the PCG iteration when every peer could be mapped
@@ -472,6 +492,7 @@ int sqnorm_dev(b200_handle* h, double* d_out);
 int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, double* d_gradient, bool want_jacobian,
                  const double* d_scale, double* cost_out, double* d_sqnorm = nullptr, bool* sqnorm_done = nullptr) {
   if (!want_jacobian) d_sqnorm = nullptr;   // the column norms are those of the stored Jacobian
+  else h->xs_ready = false;                 // S is a function of J
   EvalArgs a{};
   a.state = d_state;
   a.residuals = d_residuals;
@@ -562,8 +583,114 @@ int sqnorm_dev(b200_handle* h, double* d_out) {
 }
 
 int scale_dev(b200_handle* h, const double* d_scale) {
+  h->xs_ready = false;   // S is a function of J
   return launch(h, K_SCALE, [&] {
     scale_kernel<<<flat_grid(h, 12 * static_cast<size_t>(h->N), 256), 256, 0, h->stream>>>(h->view, d_scale);
+  });
+}
+
+// Block pattern of the upper triangle of S and what its assembly and product read (explicit_schur.cuh), built from the
+// row structure in the internal order.  Block row i: the diagonal block first (also for a camera without rows), then
+// the cameras j > i sharing a point with i in increasing order; every block lists its row pairs (r, s) in the order
+// (row r of camera i in row order, row s of r's point in row order) -- a fixed summation order.
+struct XsPattern {
+  long long off_blocks = 0;   // distinct camera pairs i < j that share a point
+  std::vector<int> blk_row, blk_col, pair_ptr, list_ptr;
+  std::vector<int2> pairs, list;
+};
+void xs_pattern(int C, int N, const int* cam_idx, const int* pt_idx, const int* pt_ptr, XsPattern* xp) {
+  std::vector<int> cptr(static_cast<size_t>(C) + 1, 0), crow(static_cast<size_t>(N));
+  for (int r = 0; r < N; ++r) cptr[cam_idx[r] + 1]++;
+  for (int c = 0; c < C; ++c) cptr[c + 1] += cptr[c];
+  {
+    std::vector<int> fill(cptr.begin(), cptr.end() - 1);
+    for (int r = 0; r < N; ++r) crow[fill[cam_idx[r]]++] = r;
+  }
+  std::vector<int> stamp(static_cast<size_t>(C), -1), slot(static_cast<size_t>(C), 0), js, start;
+  std::vector<int> row_start(static_cast<size_t>(C) + 1, 0);
+  std::vector<int3> tup;
+  for (int i = 0; i < C; ++i) {
+    js.clear();
+    tup.clear();
+    stamp[i] = i;   // the diagonal block exists even for a camera without rows
+    js.push_back(i);
+    for (int k = cptr[i]; k < cptr[i + 1]; ++k) {
+      const int r = crow[k], p = pt_idx[r];
+      for (int s = pt_ptr[p]; s < pt_ptr[p + 1]; ++s) {
+        const int j = cam_idx[s];
+        if (j < i) continue;
+        if (stamp[j] != i) {
+          stamp[j] = i;
+          js.push_back(j);
+        }
+        tup.push_back(make_int3(j, r, s));
+      }
+    }
+    std::sort(js.begin(), js.end());
+    xp->off_blocks += static_cast<long long>(js.size()) - 1;
+    row_start[i] = static_cast<int>(xp->blk_row.size());
+    start.assign(js.size() + 1, 0);
+    for (size_t t = 0; t < js.size(); ++t) {
+      slot[js[t]] = static_cast<int>(t);
+      xp->blk_row.push_back(i);
+      xp->blk_col.push_back(js[t]);
+    }
+    for (const int3& t : tup) start[slot[t.x] + 1]++;
+    for (size_t t = 0; t < js.size(); ++t) start[t + 1] += start[t];
+    const size_t base = xp->pairs.size();
+    for (size_t t = 0; t < js.size(); ++t) xp->pair_ptr.push_back(static_cast<int>(base + start[t]));
+    xp->pairs.resize(base + tup.size());
+    for (const int3& t : tup) xp->pairs[base + start[slot[t.x]]++] = make_int2(t.y, t.z);
+  }
+  const int nb = static_cast<int>(xp->blk_row.size());
+  row_start[C] = nb;
+  xp->pair_ptr.push_back(static_cast<int>(xp->pairs.size()));
+  // product lists: block row i, then the blocks (j, i) above the diagonal of column i, in order of j
+  std::vector<int> tcnt(static_cast<size_t>(C) + 1, 0);
+  for (int b = 0; b < nb; ++b)
+    if (xp->blk_col[b] != xp->blk_row[b]) tcnt[xp->blk_col[b] + 1]++;
+  for (int c = 0; c < C; ++c) tcnt[c + 1] += tcnt[c];
+  std::vector<int2> tr(static_cast<size_t>(tcnt[C]));
+  {
+    std::vector<int> fill(tcnt.begin(), tcnt.end() - 1);
+    for (int b = 0; b < nb; ++b)
+      if (xp->blk_col[b] != xp->blk_row[b])
+        tr[fill[xp->blk_col[b]]++] = make_int2(b, static_cast<int>(static_cast<uint32_t>(xp->blk_row[b]) | kXsTransposed));
+  }
+  xp->list_ptr.assign(static_cast<size_t>(C) + 1, 0);
+  xp->list.reserve(static_cast<size_t>(nb) + tr.size());
+  for (int i = 0; i < C; ++i) {
+    xp->list_ptr[i] = static_cast<int>(xp->list.size());
+    for (int b = row_start[i]; b < row_start[i + 1]; ++b) xp->list.push_back(make_int2(b, xp->blk_col[b]));
+    xp->list.insert(xp->list.end(), tr.begin() + tcnt[i], tr.begin() + tcnt[i + 1]);
+  }
+  xp->list_ptr[C] = static_cast<int>(xp->list.size());
+}
+
+// (Re)assembles S for the current implicit-Schur initialisation; also writes the diagonal blocks into d_upper45.
+// Billed as the block-diagonal operation of the elimination, which it replaces.
+int xs_assemble_dev(b200_handle* h) {
+  // the blocks with long pair lists (the diagonal ones, mostly) first, one CTA each; then one warp per block
+  OK(launch(h, K_DIAG_BLOCKS, [&] {
+    if (h->num_xs_long > 0)
+      xs_assemble_kernel<true><<<std::min(h->num_xs_long, h->sm_count * 32), kXsAsmThreads, 0, h->stream>>>(
+          h->xsv, h->view, h->d_xs_order, h->num_xs_long, h->d_ete_inv, h->d_upper45);
+    if (h->num_xs_short > 0)
+      xs_assemble_kernel<false><<<std::min((h->num_xs_short + kXsAsmThreads / 32 - 1) / (kXsAsmThreads / 32), h->sm_count * 32),
+                                  kXsAsmThreads, 0, h->stream>>>(h->xsv, h->view, h->d_xs_order + h->num_xs_long, h->num_xs_short,
+                                                                 h->d_ete_inv, h->d_upper45);
+  }));
+  h->xs_ready = true;
+  h->xs_diag_ready = true;
+  return B200_OK;
+}
+
+// y = S x (+ D_f^2 x) on the explicit S, assembled first if it is stale; y is overwritten.
+int xs_mul_dev(b200_handle* h, const double* d_x, double* d_y) {
+  if (!h->xs_ready) OK(xs_assemble_dev(h));
+  const double* Df = h->cur_D != nullptr ? h->cur_D + 3 * static_cast<size_t>(h->P) : nullptr;
+  return launch(h, K_SCHUR_MUL, [&] {
+    xs_mul_kernel<<<h->xs_grid, kXsThreads, 0, h->stream>>>(h->xsv, d_x, d_y, Df, 0, nullptr, nullptr);
   });
 }
 
@@ -577,6 +704,7 @@ int schur_init_dev(b200_handle* h, const double* d_b, const double* d_D) {
   st.ye = h->d_ye;
   CU(cudaMemsetAsync(h->d_rhs, 0, sizeof(double) * 9 * h->C, h->stream));
   h->q_from_init = false;
+  h->xs_ready = false;
   if (h->mul_v4) {
     // v4 machinery: E, F, b and the tile's D_e through the TMA slot; also writes the per-row 2x2 blocks Q_r the camera-major
     // block-diagonal pass reads (no separate pass over E for them)
@@ -666,6 +794,14 @@ int schur_mul_dev(b200_handle* h, const double* d_x, double* d_y, const int* don
 int precond_update_dev(b200_handle* h, int type) {
   if (type == B200_PRECOND_IDENTITY) return B200_OK;
   const double* Df = h->cur_D != nullptr ? h->cur_D + 3 * static_cast<size_t>(h->P) : nullptr;
+  if (h->xs && type == B200_PRECOND_SCHUR_JACOBI) {
+    // the diagonal blocks of the explicit S: no pass of their own
+    if (!h->xs_ready || !h->xs_diag_ready) OK(xs_assemble_dev(h));
+    return launch(h, K_INVERT9, [&] {
+      invert9_kernel<<<(h->C + kInvWarps - 1) / kInvWarps, 32 * kInvWarps, 0, h->stream>>>(h->C, h->d_upper45, Df, h->d_blocks, h->d_minv);
+    });
+  }
+  h->xs_diag_ready = false;
   CU(cudaMemsetAsync(h->d_upper45, 0, sizeof(double) * 45 * h->C, h->stream));
   if (h->cam_major_ok) {
     const bool schur = type == B200_PRECOND_SCHUR_JACOBI;
@@ -716,6 +852,9 @@ int schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, const 
                     b200_solver_summary* summary) {
   OK(schur_init_dev(h, d_b, d_D));
   const bool general = o->preconditioner_type == B200_PRECOND_SCHUR_POWER_SERIES_EXPANSION || o->use_spse_initialization != 0;
+  // explicit S with SCHUR_JACOBI (the configuration the reference allows use_explicit_schur_complement in): the
+  // assembly in precond_update_dev yields the preconditioner's blocks too
+  const bool explicit_s = h->xs && !general && o->preconditioner_type == B200_PRECOND_SCHUR_JACOBI;
   if (!general) OK(precond_update_dev(h, o->preconditioner_type));
   const int n = 9 * h->C;
   CgParams prm{};
@@ -756,7 +895,7 @@ int schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, const 
   };
   // In direct-flush mode the vector kernel pre-seeds the next product's output (D_f^2 p, rank 0 only) and the product
   // kernels RED straight into it: one product launch + one vector launch per iteration.
-  const bool seeded = h->v2_ok && h->v2.direct;
+  const bool seeded = (h->v2_ok && h->v2.direct) || explicit_s;
   va.Df = (h->rank == 0) ? Df : nullptr;
   // multi-GPU: the partial products travel through peer memory instead of an NCCL all-reduce (needs the direct-flush
   // product: `out` then holds exactly this rank's partial)
@@ -777,14 +916,32 @@ int schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, const 
     });
   };
   // p.q fused into the product's flush (single GPU, v4 kernel, direct flush, no separate big-point launch)
-  const bool fuse_pq = seeded && h->mul_v4 && (h->world == 1 || xchg) && h->num_huge == 0 && (h->num_big_tiles == 0 || h->big_folded) &&
+  const bool fuse_pq = (explicit_s || (seeded && h->mul_v4 && (h->world == 1 || xchg) && h->num_huge == 0 &&
+                                       (h->num_big_tiles == 0 || h->big_folded))) &&
                        dev_env("B200_NO_FUSED_PQ") == nullptr;
   double* pq_parts = fuse_pq ? h->d_pq_parts : nullptr;
   va.pq_parts = pq_parts;
-  va.num_pq_parts = fuse_pq ? h->v2.num_ctas : 0;
+  va.num_pq_parts = fuse_pq ? (explicit_s ? h->xs_grid : h->v2.num_ctas) : 0;
   va.seed_pq = fuse_pq ? h->d_seed_pq : nullptr;
   const bool use_pdl = dev_env("B200_NO_PDL") == nullptr && !h->profiling;
   auto product = [&](const double* vin, double* out) -> int {
+    if (explicit_s) {
+      // adds S vin onto the seeded output; programmatic dependent launch like the v4 product
+      return launch(h, K_SCHUR_MUL, [&] {
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(h->xs_grid);
+        cfg.blockDim = dim3(kXsThreads);
+        cfg.dynamicSmemBytes = 0;
+        cfg.stream = h->stream;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = use_pdl ? 1 : 0;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        cudaLaunchKernelEx(&cfg, xs_mul_kernel, h->xsv, vin, out, static_cast<const double*>(nullptr), 1,
+                           static_cast<const int*>(&h->d_cg->done), pq_parts);
+      });
+    }
     if (seeded) {
       // The handful of >32-row points runs on a side stream, concurrently with the warp-tile kernel (both only add
       // into the pre-seeded output with REDs); outside profiling mode, where launches are bracketed by events.
@@ -1985,6 +2142,85 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
             !h->v2_ok ? "tile" : h->mul_v4 ? (h->mul_v4_owned ? "v4-owned" : "v4") : "v3", h->v2_mul.warps, h->v2_mul.stages, h->v2_mul.replicas, h->mul_smem,
             h->big_folded ? 1 : 0, h->v2b_ok ? 1 : 0, h->cam_major_ok ? 1 : 0,
             h->cam_major_ok ? "cam_major" : (h->v2b_ok && h->diag_v2_replicas > 0) ? "v2" : "tile");
+  // Explicit or implicit S (DESIGN §1): explicit when the product on the stored upper triangle reads clearly fewer bytes
+  // than the implicit product streams and the storage fits; sharded handles stay implicit.
+  XsPattern xp;
+  double xs_mul_bytes = 0.0, xs_asm_bytes = 0.0;
+  if (h->world == 1) {
+    int l2_bytes = 0;
+    CU(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, h->device));
+    const double l2_budget = kL2ResidentShare * l2_bytes - 8.0 * (8 * 9 + 81) * C;   // as the S*x residency plan
+    xs_pattern(C, N, cam_idx, pt_idx, pt_ptr.data(), &xp);
+    const double nb = static_cast<double>(xp.blk_row.size()), npairs = static_cast<double>(xp.pairs.size());
+    const double implicit_bytes = 196.0 * N + 52.0 * P + 216.0 * C;
+    xs_mul_bytes = 648.0 * xp.list.size() + 8.0 * xp.list.size() + 216.0 * C;   // blocks as listed (off-diagonal twice), list, x, y
+    const double storage = 648.0 * nb + 8.0 * npairs + 12.0 * nb;
+    h->xs = implicit_bytes >= kXsByteRatio * xs_mul_bytes && implicit_bytes > l2_budget && storage <= kXsMaxBytes && npairs < 2.0e9;
+    if (const char* e = dev_env("B200_EXPLICIT_S")) h->xs = atoi(e) != 0 && npairs < 2.0e9;
+    // J, point of each row, (E'E+D^2)^-1, row pairs, block table; S and the diagonal upper triangles written
+    xs_asm_bytes = 196.0 * N + 48.0 * P + 8.0 * npairs + 12.0 * nb + 648.0 * nb + 360.0 * C;
+    if (getenv("B200_VERBOSE") != nullptr)
+      fprintf(stderr, "[b200ba] S plan: %s, %lld pairs, %.1f MB\n", h->xs ? "explicit" : "implicit", xp.off_blocks, 648.0 * nb / 1e6);
+  } else if (getenv("B200_VERBOSE") != nullptr) {
+    fprintf(stderr, "[b200ba] S plan: implicit, sharded\n");
+  }
+  if (h->xs) {
+    const int nb = static_cast<int>(xp.blk_row.size());
+    // product warp groups: contiguous camera ranges balanced by list length (+ a per-camera overhead)
+    const int groups_want = std::max(1, std::min(C, 4 * h->sm_count * kXsGroups));
+    h->xs_grid = (groups_want + kXsGroups - 1) / kXsGroups;
+    const int nw = h->xs_grid * kXsGroups;
+    std::vector<int> warp_cam(static_cast<size_t>(nw) + 1, C);
+    {
+      const double per_cam = 4.0;
+      const double total = static_cast<double>(xp.list.size()) + per_cam * C;
+      double cum = 0.0;
+      int w = 0;
+      for (int i = 0; i < C; ++i) {
+        const int owner = std::min(nw - 1, static_cast<int>(cum * nw / total));
+        while (w <= owner) warp_cam[w++] = i;
+        cum += (xp.list_ptr[i + 1] - xp.list_ptr[i]) + per_cam;
+      }
+      // warps past the last owner start (and end) at C
+    }
+    OK(dev_alloc(&h->d_xs_blk_row, static_cast<size_t>(nb)));
+    OK(dev_alloc(&h->d_xs_blk_col, static_cast<size_t>(nb)));
+    OK(dev_alloc(&h->d_xs_pair_ptr, static_cast<size_t>(nb) + 1));
+    OK(dev_alloc(&h->d_xs_pairs, xp.pairs.size()));
+    OK(dev_alloc(&h->d_xs_list_ptr, static_cast<size_t>(C) + 1));
+    OK(dev_alloc(&h->d_xs_list, xp.list.size()));
+    OK(dev_alloc(&h->d_xs_warp_cam, warp_cam.size()));
+    OK(dev_alloc(&h->d_xs_S, 81 * static_cast<size_t>(nb)));
+    std::vector<int> order;
+    order.reserve(static_cast<size_t>(nb));
+    for (int b = 0; b < nb; ++b)
+      if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] > kXsLongPairs) order.push_back(b);
+    h->num_xs_long = static_cast<int>(order.size());
+    for (int b = 0; b < nb; ++b)
+      if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] <= kXsLongPairs) order.push_back(b);
+    h->num_xs_short = nb - h->num_xs_long;
+    OK(dev_alloc(&h->d_xs_order, static_cast<size_t>(nb)));
+    CU(cudaMemcpyAsync(h->d_xs_order, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_blk_row, xp.blk_row.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_blk_col, xp.blk_col.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_pair_ptr, xp.pair_ptr.data(), sizeof(int) * (nb + 1), cudaMemcpyHostToDevice, h->stream));
+    if (!xp.pairs.empty())
+      CU(cudaMemcpyAsync(h->d_xs_pairs, xp.pairs.data(), sizeof(int2) * xp.pairs.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_list_ptr, xp.list_ptr.data(), sizeof(int) * (C + 1), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_list, xp.list.data(), sizeof(int2) * xp.list.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_xs_warp_cam, warp_cam.data(), sizeof(int) * warp_cam.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->xsv.C = C;
+    h->xsv.num_blocks = nb;
+    h->xsv.blk_row = h->d_xs_blk_row;
+    h->xsv.blk_col = h->d_xs_blk_col;
+    h->xsv.pair_ptr = h->d_xs_pair_ptr;
+    h->xsv.pairs = h->d_xs_pairs;
+    h->xsv.list_ptr = h->d_xs_list_ptr;
+    h->xsv.list = h->d_xs_list;
+    h->xsv.warp_cam = h->d_xs_warp_cam;
+    h->xsv.S = h->d_xs_S;
+  }
   for (int k = 0; k < K_COUNT; ++k) h->grid_tile[k] = std::max(1, std::min(h->num_tiles, h->sm_count * 4));
   h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<true>, tile_smem_bytes<3, 1>());
   h->grid_tile[K_EVAL_COST] = tile_grid(h, evaluate_kernel<false>, tile_smem_bytes<3, 1>());
@@ -2004,7 +2240,8 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     h->cg_grid = std::max(1, std::min(nblocks, per_sm * h->sm_count));
     OK(dev_alloc(&h->d_red, static_cast<size_t>(h->cg_grid) * 4));
     OK(dev_alloc(&h->d_seed_pq, static_cast<size_t>(h->cg_grid)));
-    OK(dev_alloc(&h->d_pq_parts, static_cast<size_t>(prop.multiProcessorCount)));
+    const int num_pq_parts = std::max(prop.multiProcessorCount, h->xs_grid);   // v4 or explicit-S product CTAs
+    OK(dev_alloc(&h->d_pq_parts, static_cast<size_t>(num_pq_parts)));
 #ifdef B200_WITH_NCCL
     if (h->world > 1 && h->world <= kMaxXchgRanks && dev_env("B200_NO_PEER_EXCHANGE") == nullptr) {
       // Peer exchange buffers: allocated with cudaMalloc, exported with CUDA IPC, the handles all-gathered through the NCCL
@@ -2058,7 +2295,7 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     }
 #endif
     CU(cudaMemsetAsync(h->d_seed_pq, 0, sizeof(double) * h->cg_grid, h->stream));
-    CU(cudaMemsetAsync(h->d_pq_parts, 0, sizeof(double) * prop.multiProcessorCount, h->stream));
+    CU(cudaMemsetAsync(h->d_pq_parts, 0, sizeof(double) * num_pq_parts, h->stream));
   }
 
   // Algorithmic (compulsory) bytes per launch, SURVEY §8d with this layout: J values 192 B/row + 4 B camera
@@ -2080,6 +2317,10 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   h->bytes_per_op[K_PMV_LEFT_E] = 48 * Nn + 16 * Nn + 4 * Pp + 48 * Pp;             // E cells, y, chunk boundaries, x_e read + written
   h->bytes_per_op[K_PMV_LEFT_F] = 144 * Nn + 16 * Nn + 4 * Nn + 144 * Cc;           // F cells, y, row list, x_f read + written
   h->bytes_per_op[K_MODEL_COST] = 196 * Nn + 16 * Nn + 4 * Pp + 8.0 * (3 * Pp + 9 * Cc);
+  if (h->xs) {   // explicit S: the product and the assembly that replaces the block-diagonal pass
+    h->bytes_per_op[K_SCHUR_MUL] = xs_mul_bytes;
+    h->bytes_per_op[K_DIAG_BLOCKS] = xs_asm_bytes;
+  }
   return B200_OK;
 }
 
@@ -2098,6 +2339,7 @@ void b200_destroy(b200_handle* h) {
                       h->d_minv, h->d_blocks, h->d_xr, h->d_p, h->d_r, h->d_z, h->d_tmp, h->d_sol, h->d_cg,
                       h->d_scale, h->d_sqnorm, h->d_diagonal, h->d_lmD, h->d_step, h->d_cand, h->d_y, h->d_wtiles,
                       h->d_row_meta, h->d_cta_part, h->d_cta_cam, h->d_cta_cams, h->d_cta_big, h->d_cta_big_none, h->d_tile_meta, h->d_pq_parts, h->d_seed_pq, h->d_huge_pts, h->d_dense_s, h->d_dense_work, h->d_dense_info, h->d_ftf_inv, h->d_spse[0], h->d_spse[1], h->d_spse[2], h->d_partials, h->d_ybig, h->d_red, h->d_cam_items, h->d_cam_rows, h->d_q3, h->d_pt_perm, h->d_row_perm, h->d_stage_p, h->d_stage_r,
+                      h->d_xs_blk_row, h->d_xs_blk_col, h->d_xs_pair_ptr, h->d_xs_list_ptr, h->d_xs_warp_cam, h->d_xs_order, h->d_xs_pairs, h->d_xs_list, h->d_xs_S,
                       const_cast<TileDesc*>(h->view_big.tiles)};
   for (void* p : dev_ptrs)
     if (p != nullptr) cudaFree(p);
@@ -2343,6 +2585,7 @@ int b200_jacobian_get_values(b200_handle* h, double* values) {
 int b200_jacobian_set_values(b200_handle* h, const double* values) {
   if (h == nullptr || values == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   CU(cudaSetDevice(h->device));
+  h->xs_ready = false;   // S is a function of J
   const size_t n = static_cast<size_t>(h->N);
   if (!h->permuted) {
     OK(h2d(h, h->d_values, values, sizeof(double) * 24 * n));
@@ -2425,7 +2668,8 @@ int b200_schur_multiply(b200_handle* h, const double* x, double* y) {
   if (h == nullptr || x == nullptr || y == nullptr || !h->schur_ready) return fail(B200_ERR_INVALID_ARGUMENT, "b200_schur_init first");
   CU(cudaSetDevice(h->device));
   OK(h2d(h, h->d_xr, x, sizeof(double) * 9 * h->C));
-  OK(schur_mul_dev(h, h->d_xr, h->d_tmp, nullptr));
+  if (h->xs) OK(xs_mul_dev(h, h->d_xr, h->d_tmp));
+  else OK(schur_mul_dev(h, h->d_xr, h->d_tmp, nullptr));
   return d2h(h, y, h->d_tmp, sizeof(double) * 9 * h->C);
 }
 int b200_schur_back_substitute(b200_handle* h, const double* z, double* y) {
