@@ -32,8 +32,7 @@ struct V2View {
   const int2* cta_big;       // per CTA: [begin, end) into big_tiles: the >32-row points inside its row range
   const TileDesc* big_tiles; // one point each, 33..kTile rows
   const uint32_t* tile_meta; // v4: [num tiles][kV4MetaWords] row words + own descriptor + descriptor of the tile that reuses the stage
-  int stage_x;               // v4: the CTA keeps x of its camera range in shared memory
-  double* partials;          // [num_ctas][9 * max_cam_span]
+  double* partials;         // [num_ctas][9 * max_cam_span]
   int num_ctas;
   int max_cam_span;
   int warps;                 // warps per CTA
@@ -41,7 +40,6 @@ struct V2View {
   int replicas;              // copies of the private camera vector (warp w uses copy w % replicas)
   int direct;                // 1: CTAs RED their (narrow) camera range straight into the output vector; 0: partials
   int per_warp_bytes;
-  int variant;               // development builds only (-DB200_DEV_KNOBS): selects kernel variants for A/B runs; 0 in the product
   // L2 residency plan of S*x (b200_create), the same for every CTA: a fraction l2_stream / 65536 of its tiles, spread
   // evenly over its tile range, is copied with evict_first; the rest with evict_normal (evict_last if l2_last, development
   // builds), so that it stays in L2 from one product of a PCG to the next.  0: every copy evict_normal, the default policy.
@@ -496,7 +494,7 @@ constexpr int kV4StageBytes = 32 * 144 + 32 * 48 + 32 * 48 + kV4MetaWords * 4;  
 __host__ __device__ inline int v4_bars_offset(int stages) { return stages * kV4StageBytes + 32 * kV2Scratch * 8; }
 __host__ __device__ inline int v4_extra_offset(int stages) { return v4_bars_offset(stages) + ((8 * stages + 15) & ~15); }
 __host__ __device__ inline int v4_per_warp_bytes(int stages) { return v4_extra_offset(stages) + 16; }
-__host__ __device__ inline size_t v4_sx_bytes(int max_cam_span, int stage_x) { return stage_x ? v2_sy_stride(max_cam_span) * 8 : 0; }
+__host__ __device__ inline size_t v4_sx_bytes(int max_cam_span) { return v2_sy_stride(max_cam_span) * 8; }
 
 // `part_begin`: first tile of the CTA's range (the residency plan is indexed by the position of the tile inside it).
 __device__ __forceinline__ void v4_issue(const V2View& v, const double* ete_inv, unsigned char* stage, uint64_t* bar, int tile,
@@ -564,7 +562,7 @@ __device__ __forceinline__ V4Ctx v4_ctx(const V2View& v) {
   const int warp = threadIdx.x >> 5;
   c.sy_stride = static_cast<int>(v2_sy_stride(v.max_cam_span));
   c.sx_off = static_cast<int>(v2_sy_bytes(v.max_cam_span, v.replicas));
-  c.ring_off = c.sx_off + static_cast<int>(v4_sx_bytes(v.max_cam_span, 1));
+  c.ring_off = c.sx_off + static_cast<int>(v4_sx_bytes(v.max_cam_span));
   c.wbase_off = c.ring_off + warp * v.per_warp_bytes;
   c.sW_off = c.wbase_off + v.stages * kV4StageBytes;
   c.bars_off = c.sW_off + 32 * kV2Scratch * 8;

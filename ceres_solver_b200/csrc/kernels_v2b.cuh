@@ -1,5 +1,5 @@
-// Warp-tile (v2) versions of the once-per-LM-iteration kernels: evaluate (+ fused column norms), implicit-Schur
-// init (E'E inverse, rhs) and the block diagonal of the Schur complement.  Same structure as kernels_v2.cuh: one
+// Warp-tile (v2) versions of the once-per-LM-iteration kernels: evaluate (+ fused column norms) and the block diagonal
+// of the Schur complement.  Same structure as kernels_v2.cuh: one
 // persistent CTA per SM, whole points in <= 32-row warp tiles, per-point sums through __syncwarp + a per-warp
 // scratch, camera-sized results accumulated in CTA-private shared memory after a warp-level pre-reduction and
 // flushed with a few hundred REDs per CTA.  Used when the CTAs' camera ranges are narrow (V2View::direct); the
@@ -282,105 +282,6 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
   }
   if (a.gradient != nullptr) v2_flush(v, cr, sg_acc, 9, v.replicas, rstride, a.gradient + camoff);
   if (a.sqnorm != nullptr) v2_flush(v, cr, sq_acc, 9, v.replicas, rstride, a.sqnorm + camoff);
-}
-
-// ------------------------------------------------------------------------------------------------
-// ImplicitSchurComplement::Init:  ete_inv[k] = (sum E'E + D_k^2)^-1 ;  ye = ete_inv E'b ;  rhs += F'(b - E ye)
-// (rhs camera vector zeroed by the caller).  F through the per-warp TMA ring, E / b read directly.
-// ------------------------------------------------------------------------------------------------
-constexpr int kInitScratch = 9;
-
-__global__ void __launch_bounds__(kV2MaxThreads, 1) schur_init_v2_kernel(V2View v, SchurState st) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  double* sy = reinterpret_cast<double*>(smem_raw);
-  const WarpCtx c = v2_warp_ctx(v, smem_raw, kInitScratch);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int2 part = v.cta_part[blockIdx.x];
-  const int2 cr = v.cta_cam[blockIdx.x];
-  int t_issue;
-  v2_prologue(v, sy, c, part, cr, t_issue);
-  double* my_y = sy + (warp % v.replicas) * v2_sy_stride(v.max_cam_span);
-  int it = 0;
-  for (int tile = part.x + warp; tile < part.y; tile += v.warps, ++it) {
-    const int s = it % v.stages;
-    const uint32_t parity = (it / v.stages) & 1;
-    const WarpTile wt = v.wtiles[tile];
-    const bool active = lane < wt.row_count;
-    const size_t row = static_cast<size_t>(wt.row_begin) + lane;
-    const uint32_t meta = active ? __ldg(v.row_meta + row) : 0u;
-    const int cam = meta_cam(meta), cam_l = meta_local(v, meta, cr);
-    const Seg sg = v2_segment(active && meta_head(meta), wt.row_count);
-    double2 e0 = make_double2(0, 0), e1 = e0, e2 = e0;
-    double b0 = 0.0, b1 = 0.0;
-    size_t pt = 0;
-    if (active) {
-      const double2* ep = reinterpret_cast<const double2*>(v.p.E() + 6 * row);
-      e0 = __ldg(ep);
-      e1 = __ldg(ep + 1);
-      e2 = __ldg(ep + 2);
-      const double2 bb = *reinterpret_cast<const double2*>(st.b + 2 * row);
-      b0 = bb.x;
-      b1 = bb.y;
-      pt = static_cast<size_t>(wt.pt_begin + sg.lpt);
-    }
-    double in[9], m[9];
-    in[0] = e0.x * e0.x + e1.y * e1.y;
-    in[1] = e0.x * e0.y + e1.y * e2.x;
-    in[2] = e0.x * e1.x + e1.y * e2.y;
-    in[3] = e0.y * e0.y + e2.x * e2.x;
-    in[4] = e0.y * e1.x + e2.x * e2.y;
-    in[5] = e1.x * e1.x + e2.y * e2.y;
-    in[6] = e0.x * b0 + e1.y * b1;
-    in[7] = e0.y * b0 + e2.x * b1;
-    in[8] = e1.x * b0 + e2.y * b1;
-    v2_point_sum<9>(c.sW, sg, active, in, m);
-    double t0 = 0.0, t1 = 0.0;
-    if (active) {
-      if (st.D != nullptr) {
-        const double d0 = st.D[3 * pt], d1 = st.D[3 * pt + 1], d2 = st.D[3 * pt + 2];
-        m[0] += d0 * d0;
-        m[3] += d1 * d1;
-        m[5] += d2 * d2;
-      }
-      double inv[6];
-      invert_sym3_llt(m, inv);
-      const double v0 = inv[0] * m[6] + inv[1] * m[7] + inv[2] * m[8];
-      const double v1 = inv[1] * m[6] + inv[3] * m[7] + inv[4] * m[8];
-      const double v2 = inv[2] * m[6] + inv[4] * m[7] + inv[5] * m[8];
-      if (lane == sg.first) {
-#pragma unroll
-        for (int k = 0; k < 6; ++k) st.ete_inv[6 * pt + k] = inv[k];
-        if (st.ye != nullptr) {
-          st.ye[3 * pt] = v0;
-          st.ye[3 * pt + 1] = v1;
-          st.ye[3 * pt + 2] = v2;
-        }
-      }
-      t0 = b0 - (e0.x * v0 + e0.y * v1 + e1.x * v2);
-      t1 = b1 - (e1.y * v0 + e2.x * v1 + e2.y * v2);
-    }
-    mbar_wait(c.bars + s, parity);
-    double g[9];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g[k] = 0.0;
-    if (active) {
-      const double* fr = c.sF + s * 576 + lane * 18;
-      double f[18];
-#pragma unroll
-      for (int k = 0; k < 9; ++k) {
-        const double2 w = lds2(fr + 2 * k);
-        f[2 * k] = w.x;
-        f[2 * k + 1] = w.y;
-      }
-#pragma unroll
-      for (int k = 0; k < 9; ++k) g[k] = f[k] * t0 + f[9 + k] * t1;
-    }
-    cam_accumulate<9>(my_y, cam_l, active, g);
-    __syncwarp();
-    if (t_issue < part.y && lane == 0) v2_issue(v, c, t_issue, s);
-    t_issue += v.warps;
-  }
-  v2_epilogue(v, sy, cr, st.rhs);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """b200_create picks its kernels from the problem's structure (the shared-memory arithmetic on the per-CTA camera span
-in b200ba.cu), and each choice is a different kernel, or a different combination of kernels writing into the same
+in plan_kernels, csrc/plan.cuh), and each choice is a different kernel, or a different combination of kernels writing into the same
 output.  One fixture per configuration, each checked through every entry point and three LM iterations against the
 oracle (tests/entry_points.py), and each asserting the configuration it got from the `[b200ba] C=...` line
 (B200_VERBOSE), so that a change of the planning heuristics fails here instead of quietly moving coverage.

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Development build of the SAME source with the A/B knobs compiled in (-DB200_DEV_KNOBS: dev_env() in b200ba.cu reads the
+# Development build of the SAME source with the A/B knobs compiled in (-DB200_DEV_KNOBS: DevKnobs in plan.cuh reads the
 # B200_* variables listed in DESIGN.md's appendix).  A/B scripts load it through B200BA_LIB; the
 # product library (built by __graft_entry__.build()) reads none of them.
 set -e
