@@ -637,6 +637,7 @@ struct MulOpts {
   const int* done = nullptr;    // device flag: every launch is a no-op once the PCG has terminated
   double* pq_parts = nullptr;   // per-CTA partials of p.q, fused into the flush of the v4 and explicit-S products
   bool exchange = false;        // the vector kernel sums the ranks' partial products over peer memory: no all-reduce
+  bool xs_columns_in_cg = false;  // explicit S: the PCG's vector kernel adds the column part from T (no gather launch)
 };
 
 // y = S x on device vectors [9C], with S = F'F + D_f^2 - F'E (E'E + D_e^2)^-1 E'F of the current initialisation.
@@ -644,10 +645,14 @@ int schur_mul_dev(b200_handle* h, const double* d_x, double* d_y, const MulOpts&
   const double* Df = h->cur_D != nullptr ? h->cur_D + 3 * static_cast<size_t>(h->P) : nullptr;
   if (o.explicit_s) {
     if (!h->xs_ready) OK(xs_assemble_dev(h));
-    return launch(h, K_SCHUR_MUL, [&] {
+    OK(launch(h, K_SCHUR_MUL, [&] {
       launch_pdl(xs_mul_kernel, h->xs_grid, kXsThreads, 0, h->stream, o.pdl, h->xsv, d_x, d_y, o.seeded ? nullptr : Df,
                  o.seeded ? 1 : 0, o.done, o.pq_parts);
-    });
+    }));
+    if (o.xs_columns_in_cg) return B200_OK;
+    return launch(h, K_SCHUR_MUL, [&] {
+      xs_gather_kernel<<<(9 * h->C + 255) / 256, 256, 0, h->stream>>>(h->xsv, d_y);
+    }, false);
   }
   const int n = 9 * h->C;
   const double* seed = (h->rank == 0) ? Df : nullptr;
@@ -836,6 +841,9 @@ int schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, const 
   mo.done = &h->d_cg->done;
   mo.pq_parts = fuse_pq ? h->d_pq_parts : nullptr;
   mo.exchange = xchg;
+  mo.xs_columns_in_cg = explicit_s;
+  va.xs_col_ptr = explicit_s ? h->xsv.col_ptr : nullptr;
+  va.xs_T = explicit_s ? h->xsv.T : nullptr;
   va.pq_parts = mo.pq_parts;
   va.num_pq_parts = fuse_pq ? (explicit_s ? h->xs_grid : h->v2.num_ctas) : 0;
   va.seed_pq = fuse_pq ? h->d_seed_pq : nullptr;
@@ -1307,7 +1315,9 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   OK(validate_rows(desc, &caller_ptr));
   int l2_bytes = 0;
   CU(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, desc->device));
-  const DevLimits lim{prop.multiProcessorCount, prop.sharedMemPerBlockOptin, l2_bytes};
+  int xs_per_sm = 0;   // the explicit-S product's grid is one wave of these (plan.cuh)
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&xs_per_sm, xs_mul_kernel, kXsThreads, 0));
+  const DevLimits lim{prop.multiProcessorCount, prop.sharedMemPerBlockOptin, l2_bytes, xs_per_sm};
   const DevKnobs knobs = DevKnobs::from_env();
   const int world = desc->world_size > 1 ? desc->world_size : 1;
   KernelPlan pl;
@@ -1456,10 +1466,12 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     OK(upload(h, xp.blk_col, &x.blk_col));
     OK(upload(h, xp.pair_ptr, &x.pair_ptr));
     OK(upload(h, xp.pairs, &x.pairs));
-    OK(upload(h, xp.list_ptr, &x.list_ptr));
-    OK(upload(h, xp.list, &x.list));
-    OK(upload(h, pl.xs_warp_cam, &x.warp_cam));
+    OK(upload(h, xp.cols, &x.cols));
+    OK(upload(h, xp.col_ptr, &x.col_ptr));
+    OK(upload(h, pl.xs_steps, &x.steps));
+    OK(upload(h, pl.xs_warp_step, &x.warp_step));
     OK(dev_alloc(h, &x.S, 81 * static_cast<size_t>(x.num_blocks)));
+    OK(dev_alloc(h, &x.T, 9 * static_cast<size_t>(xp.off_blocks)));
     OK(upload(h, pl.xs_order, &h->d_xs_order));
     h->num_xs_long = pl.num_xs_long;
     h->num_xs_short = x.num_blocks - pl.num_xs_long;

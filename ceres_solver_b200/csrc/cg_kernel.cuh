@@ -16,6 +16,7 @@
 #pragma once
 #include <cooperative_groups.h>
 
+#include "explicit_schur.cuh"
 #include "vector_kernels.cuh"
 
 namespace b200 {
@@ -70,6 +71,10 @@ struct CgVecArgs {
   const double* minv;
   const double* rhs;
   double *x, *r, *z, *p, *q;   // q holds S*p (S*x_new in CG_RESET_SECOND)
+  // explicit S (explicit_schur.cuh): q holds the product's row part; its column part is summed here from T (xs_col_sum).
+  // Null: q is complete.
+  const int* xs_col_ptr;
+  const double* xs_T;
   double* red;                 // [gridDim.x][4] partial sums
   CgState* st;
   // p.q without a pass over q (single GPU, direct-flush products): pq_parts[0..num_pq_parts) hold p . (partial of S0 p)
@@ -183,7 +188,12 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
       for (int b = lane; b < static_cast<int>(gridDim.x); b += 32) pq_pre += __ldcg(a.seed_pq + b);
     }
   }
-  if (ok0 && mode != CG_BEGIN && a.xg.world <= 1) qj = __ldcg(a.q + j0);
+  // q of entry j: the product's output, plus the column part of an explicit-S product
+  auto load_q = [&](int j) -> double {
+    const double q = __ldcg(a.q + j);
+    return a.xs_T != nullptr ? xs_col_sum(a.xs_col_ptr, a.xs_T, j, q) : q;
+  };
+  if (ok0 && mode != CG_BEGIN && a.xg.world <= 1) qj = load_q(j0);
 
   if (mode != CG_BEGIN && st_done) return;
   if (a.xg.world > 1 && mode != CG_BEGIN) {
@@ -212,7 +222,7 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
     } else {
       for (int blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
         const int j = blk * kCgCamsPerCta * 9 + tid;
-        if (lane_ok && j < n) acc += a.p[j] * a.q[j];
+        if (lane_ok && j < n) acc += a.p[j] * load_q(j);
       }
     }
     cg_block_sum3(acc, d1, d2, scratch);
@@ -282,7 +292,7 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
         bj = a.rhs[j];
         if (mode != CG_BEGIN) {
           pj = a.p[j];
-          qj = a.q[j];
+          qj = load_q(j);
           xj = a.x[j];
           if (mode != CG_RESET_SECOND) rj = a.r[j];
         }

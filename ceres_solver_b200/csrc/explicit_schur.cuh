@@ -15,9 +15,11 @@
 // its transpose).  One warp owns one block, or one CTA a block with many pairs (the diagonal blocks): no atomics, fixed
 // summation order, plain stores.
 //
-// Product.  Each output camera i owns y_i = sum_{j >= i} S_ij x_j + sum_{j < i} S_ji' x_j: a pair of warps walks the list
-// of block row i followed by the blocks of column i above the diagonal (each off-diagonal block is read twice, from a
-// footprint that is half of the full matrix), accumulates with fixed order and writes y_i once.
+// Product (one pass over the stored triangle).  The warp that owns block row i streams it once, three blocks per step
+// (lane 9e + w holds column w of the step's block e, lanes 27..31 idle).  For each block (i, j) it adds S_ij x_j into
+// the row part a_i, and for j > i it also forms t_ij = S_ij' x_i, which it stores in the block's slot of T.  It writes
+// y_i = seed + a_i; the column part sum_{i<j} t_ij of q_j is added by whoever reads q next: the PCG's vector kernel
+// (xs_col_sum) or, outside the PCG, xs_gather_kernel.  T is ordered by column, so that sum reads contiguous slots.
 #pragma once
 #include "common.cuh"
 
@@ -25,12 +27,14 @@ namespace b200 {
 
 constexpr int kXsThreads = 256;       // product: 8 warps per CTA
 constexpr int kXsWarps = kXsThreads / 32;
-constexpr int kXsSplit = 2;           // warps per output camera
-constexpr int kXsGroups = kXsWarps / kXsSplit;   // groups of kXsSplit warps per CTA, each owning a contiguous camera range
-constexpr int kXsBatch = 4;           // blocks in flight per warp in the product
+constexpr int kXsMinCtas = 2;         // product CTAs per SM its register budget (__launch_bounds__) is sized for
+constexpr int kXsStep = 3;            // blocks per product step: lane 9e + w owns column w of block e
 constexpr int kXsAsmThreads = 256;    // assembly: one warp per block, or one CTA per block with a long pair list
 constexpr int kXsLongPairs = 96;      // ... longer than this
-constexpr uint32_t kXsTransposed = 0x80000000u;
+// product step descriptor {first block, row | count << 27 | first of row | last of row}
+constexpr int kXsStepCountShift = 27;
+constexpr int kXsStepFirst = 1 << 29;
+constexpr int kXsStepLast = 1 << 30;
 
 struct XsView {
   int C;
@@ -39,10 +43,12 @@ struct XsView {
   const int* blk_col;        // [num_blocks] j
   const int* pair_ptr;       // [num_blocks + 1] row pairs of each block
   const int2* pairs;         // (r, s): cam r = i, cam s = j, same point
-  const int* list_ptr;       // [C + 1] product list of output camera i
-  const int2* list;          // {block, j | kXsTransposed when the block is (j, i), j < i}
-  const int* warp_cam;       // [groups + 1] first output camera of each product warp group
+  const int2* cols;          // [num_blocks] {j, T slot of the block; -1 for a diagonal block}
+  const int* col_ptr;        // [C + 1] T slots of column j: its blocks (i, j), i < j, in order of i
+  const int2* steps;         // product steps, each warp's in order (descriptor above)
+  const int* warp_step;      // [warps + 1] first step of each product warp
   double* S;                 // [num_blocks][81]
+  double* T;                 // [pairs][9] t_ij = S_ij' x_i of the last product, by T slot
 };
 
 // Row pairs [q_begin, q_end) of one block into the lane's entries (u, w0 .. w0 + 2); lanes 0..26 own entries.  G of 8
@@ -159,91 +165,103 @@ __global__ void __launch_bounds__(kXsAsmThreads) xs_assemble_kernel(XsView v, Pr
   }
 }
 
-// y = [y if accumulate] + [D_f^2 x if Df] + S x, S as assembled (without D_f^2).  Inside the PCG: accumulate onto the
-// output the vector kernel seeded, no-op once done_flag is set, and pq_part[CTA] = x . (this CTA's rows of S x) -- the
-// product protocol of schur_mul_v4_kernel.  Launched with programmatic stream serialisation behind the vector kernel.
-// kXsSplit warps share each output camera (alternate batches of its list) and add their sums in warp order.
-__global__ void __launch_bounds__(kXsThreads, 3) xs_mul_kernel(XsView v, const double* __restrict__ x, double* y,
-                                                               const double* __restrict__ Df, int accumulate,
-                                                               const int* __restrict__ done_flag, double* pq_part) {
-  __shared__ double s_acc[kXsWarps][2][81];
+// The lane's column of the blocks of one product step and the column entry it reads them with.
+struct XsStepData {
+  int2 d;        // step descriptor
+  int2 c;        // {j, T slot} of the lane's block ({0, -1}: no block)
+  double s[9];   // S[u][w] of the lane's block, u = 0..8
+};
+__device__ __forceinline__ int2 xs_step_desc(const XsView& v, int k, int k1) {
+  return k < k1 ? __ldg(v.steps + k) : make_int2(0, 0);   // past the end: a step of no blocks
+}
+__device__ __forceinline__ bool xs_lane_in(int2 d, int e) { return e < ((d.y >> kXsStepCountShift) & 3); }
+__device__ __forceinline__ int2 xs_step_col(const XsView& v, int2 d, int e) {
+  return xs_lane_in(d, e) ? __ldg(v.cols + d.x + e) : make_int2(0, -1);
+}
+__device__ __forceinline__ void xs_step_s(const XsView& v, int2 d, int e, int w, double* s) {
+  const bool in = xs_lane_in(d, e);
+  const int b = in ? d.x + e : 0;
+  const double* sb = v.S + 81 * static_cast<size_t>(b) + w;
+#pragma unroll
+  for (int u = 0; u < 9; ++u) s[u] = in ? __ldg(sb + 9 * u) : 0.0;
+}
+
+// y = [y if accumulate] + [D_f^2 x if Df] + (row part of S x), and T = the column part (file comment), S as assembled
+// (without D_f^2).  Inside the PCG: accumulate onto the output the vector kernel seeded, no-op once done_flag is set, and
+// pq_part[CTA] = sum over this CTA's rows of x_i . a_i + sum over its off-diagonal blocks of x_j . t_ij, i.e. its share of
+// x . S x -- the product protocol of schur_mul_v4_kernel.  Launched with programmatic stream serialisation behind the
+// vector kernel: the steps, column entries and S of the first two steps are static and are read before the wait.
+// Each warp walks its steps with the next step's S and x_j in flight and the column entries of the one after.
+__global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v, const double* __restrict__ x, double* y,
+                                                                        const double* __restrict__ Df, int accumulate,
+                                                                        const int* __restrict__ done_flag, double* pq_part) {
   __shared__ double s_pq[kXsWarps];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int grp = warp / kXsSplit, h = warp - kXsSplit * grp;
-  const int gid = blockIdx.x * kXsGroups + grp;
-  // static data first: it may be read before the kernel that produces x has finished
-  const int c0 = __ldg(v.warp_cam + gid), c1 = __ldg(v.warp_cam + gid + 1);
+  const int e = lane / 9, w = lane - 9 * (lane / 9);   // e == 3: lanes 27..31, no block
+  const int gw = blockIdx.x * kXsWarps + warp;
+  const int k0 = __ldg(v.warp_step + gw), k1 = __ldg(v.warp_step + gw + 1);
+  XsStepData nx;   // step k + 1
+  nx.d = xs_step_desc(v, k0, k1);
+  nx.c = xs_step_col(v, nx.d, e);
+  xs_step_s(v, nx.d, e, w, nx.s);
+  int2 d2 = xs_step_desc(v, k0 + 1, k1), c2 = xs_step_col(v, d2, e);   // step k + 2: descriptor and column entry
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (done_flag != nullptr && __ldcg(done_flag) != 0) return;
-  // lane entries k = lane + 32 m of a block: row u_m, column w_m (m = 2 only for lanes < 17)
-  const bool ok2 = lane < 17;
-  int um[3], wm[3];
+  double nx_x = xs_lane_in(nx.d, e) ? __ldcg(x + 9 * static_cast<size_t>(nx.c.x) + w) : 0.0;
+  double acc[9], xi[9];
 #pragma unroll
-  for (int m = 0; m < 3; ++m) {
-    const int k = (m < 2 || ok2) ? lane + 32 * m : 0;
-    um[m] = k / 9;
-    wm[m] = k - 9 * (k / 9);
-  }
+  for (int u = 0; u < 9; ++u) acc[u] = xi[u] = 0.0;
   double pq = 0.0;
-  for (int i = c0; i < c1; ++i) {
-    double a[3] = {0.0, 0.0, 0.0};   // sum over blocks (i, j) of S_ij[u][w] x_j[w]  -> y_i[u]
-    double t[3] = {0.0, 0.0, 0.0};   // sum over blocks (j, i) of S_ji[u][w] x_j[u]  -> y_i[w]
-    const int l0 = __ldg(v.list_ptr + i), l1 = __ldg(v.list_ptr + i + 1);
-    for (int l = l0 + h * kXsBatch; l < l1; l += kXsBatch * kXsSplit) {
-      double sv[kXsBatch][3], xv[kXsBatch][3];
-      unsigned tr = 0u;   // bit e: entry e is a transposed block
+  for (int k = k0; k < k1; ++k) {
+    const int2 d = nx.d, c = nx.c;
+    double s[9];
 #pragma unroll
-      for (int e = 0; e < kXsBatch; ++e) {
-        const bool ok = l + e < l1;
-        const int2 ent = ok ? __ldg(v.list + l + e) : make_int2(0, 0);
-        const bool te = (static_cast<uint32_t>(ent.y) & kXsTransposed) != 0;
-        tr |= te ? 1u << e : 0u;
-        const int j = static_cast<int>(static_cast<uint32_t>(ent.y) & ~kXsTransposed);
-        const double* sb = v.S + 81 * static_cast<size_t>(ent.x);
-        const double* xj = x + 9 * static_cast<size_t>(j);
+    for (int u = 0; u < 9; ++u) s[u] = nx.s[u];
+    const double xj = nx_x;
+    // refill: step k + 1 from the entries loaded one step ago, the column entries of step k + 2
+    nx.d = d2;
+    nx.c = c2;
+    xs_step_s(v, nx.d, e, w, nx.s);
+    nx_x = xs_lane_in(nx.d, e) ? __ldcg(x + 9 * static_cast<size_t>(nx.c.x) + w) : 0.0;
+    d2 = xs_step_desc(v, k + 2, k1);
+    c2 = xs_step_col(v, d2, e);
+    // a row begins with its diagonal block in lanes 0..8: their x_j is x_i
+    if (d.y & kXsStepFirst)
 #pragma unroll
-        for (int m = 0; m < 3; ++m) {
-          const bool use = ok && (m < 2 || ok2);
-          sv[e][m] = use ? __ldg(sb + lane + 32 * m) : 0.0;
-          xv[e][m] = use ? __ldcg(xj + (te ? um[m] : wm[m])) : 0.0;
-        }
-      }
+      for (int u = 0; u < 9; ++u) xi[u] = __shfl_sync(0xffffffffu, xj, u);
+    double t = 0.0;
 #pragma unroll
-      for (int e = 0; e < kXsBatch; ++e)
-#pragma unroll
-        for (int m = 0; m < 3; ++m) {
-          const double prod = sv[e][m] * xv[e][m];
-          if ((tr >> e) & 1u) t[m] += prod;
-          else a[m] += prod;
-        }
+    for (int u = 0; u < 9; ++u) {
+      acc[u] += s[u] * xj;   // lanes without a block hold s = 0, x_j = 0
+      t += s[u] * xi[u];
     }
-#pragma unroll
-    for (int m = 0; m < 3; ++m)
-      if (m < 2 || ok2) {
-        s_acc[warp][0][lane + 32 * m] = a[m];
-        s_acc[warp][1][lane + 32 * m] = t[m];
-      }
-    // the warps of the group meet on a named barrier (id 1 + group; 0 is __syncthreads)
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(32 * kXsSplit) : "memory");
-    if (h == 0 && lane < 9) {
-      double acc = 0.0;
-#pragma unroll
-      for (int hh = 0; hh < kXsSplit; ++hh) {
-        const double(*sa)[81] = s_acc[kXsSplit * grp + hh];
-#pragma unroll
-        for (int w = 0; w < 9; ++w) acc += sa[0][9 * lane + w];
-#pragma unroll
-        for (int uu = 0; uu < 9; ++uu) acc += sa[1][9 * uu + lane];
-      }
-      const size_t o = 9 * static_cast<size_t>(i) + lane;
-      const double xo = __ldcg(x + o);
-      pq += xo * acc;
-      double out = acc;
-      if (Df != nullptr) out += Df[o] * Df[o] * xo;
-      if (accumulate) out += __ldcg(y + o);
-      y[o] = out;
+    if (c.y >= 0) {
+      v.T[9 * static_cast<size_t>(c.y) + w] = t;
+      pq += xj * t;
     }
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(32 * kXsSplit) : "memory");
+    if (d.y & kXsStepLast) {
+      // a_i[u] = sum over the lanes of acc[u]: a butterfly, so every lane holds the same bits
+      double mine = 0.0, xo = 0.0;
+#pragma unroll
+      for (int u = 0; u < 9; ++u) {
+        double a = acc[u];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == u) {
+          mine = a;
+          xo = xi[u];
+        }
+        acc[u] = 0.0;
+      }
+      if (lane < 9) {
+        const size_t o = 9 * static_cast<size_t>(d.y & ((1 << kXsStepCountShift) - 1)) + lane;
+        pq += xo * mine;
+        double out = mine;
+        if (Df != nullptr) out += Df[o] * Df[o] * xo;
+        if (accumulate) out += __ldcg(y + o);
+        y[o] = out;
+      }
+    }
   }
   if (pq_part == nullptr) return;
 #pragma unroll
@@ -253,9 +271,31 @@ __global__ void __launch_bounds__(kXsThreads, 3) xs_mul_kernel(XsView v, const d
   if (threadIdx.x == 0) {
     double tot = 0.0;
 #pragma unroll
-    for (int w = 0; w < kXsWarps; ++w) tot += s_pq[w];
+    for (int ww = 0; ww < kXsWarps; ++ww) tot += s_pq[ww];
     pq_part[blockIdx.x] = tot;
   }
+}
+
+// q + the column part of entry k = 9j + w of S x: sum over the blocks (i, j), i < j, of t_ij[w] in order of i (their T
+// slots are contiguous), loaded 8 at a time.
+__device__ __forceinline__ double xs_col_sum(const int* __restrict__ col_ptr, const double* T, int k, double q) {
+  const int j = k / 9, w = k - 9 * (k / 9);
+  const int c0 = __ldg(col_ptr + j), c1 = __ldg(col_ptr + j + 1);
+  for (int c = c0; c < c1; c += 8) {
+    double t[8];
+#pragma unroll
+    for (int m = 0; m < 8; ++m) t[m] = c + m < c1 ? __ldcg(T + 9 * static_cast<size_t>(c + m) + w) : 0.0;
+#pragma unroll
+    for (int m = 0; m < 8; ++m)
+      if (c + m < c1) q += t[m];
+  }
+  return q;
+}
+
+// Completes a product outside the PCG: y += the column part held in T.
+__global__ void __launch_bounds__(256) xs_gather_kernel(XsView v, double* y) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < 9 * v.C) y[k] = xs_col_sum(v.col_ptr, v.T, k, y[k]);
 }
 
 }  // namespace b200

@@ -21,8 +21,9 @@ namespace b200 {
 // Share of the L2 the S*x residency plan may fill.  On an H100 (50 MB L2) the product got faster up to ~24 MB resident
 // and slower again from 32 MB on (DESIGN §3.2).
 constexpr double kL2ResidentShare = 0.5;
-// Explicit S (explicit_schur.cuh) when the implicit product's stream is at least kXsByteRatio times the bytes of a
-// product on the explicit upper triangle (each off-diagonal block read twice), does not fit the L2 residency budget
+// Explicit S (explicit_schur.cuh) when the implicit product's stream is at least kXsByteRatio times 656 (C + 2 pairs) +
+// 216 C bytes (the cost of a product that reads every off-diagonal block twice, the yardstick the thresholds were
+// measured against; the product now reads each block once), does not fit the L2 residency budget
 // (then the implicit product is served from L2 and the assembly cannot pay for itself), and S with its row-pair list
 // fits kXsMaxBytes (the assembly time grows with the row pairs, and a solve of few CG iterations cannot repay it).
 // Measured on one H100 (DESIGN §3): Ladybug-1723 (ratio 3.3, 40 MB) is faster explicit; ladybug-1723-random (ratio 0.47),
@@ -118,6 +119,7 @@ struct DevLimits {
   int sm_count;
   size_t smem_optin;   // cudaDeviceProp::sharedMemPerBlockOptin
   int l2_bytes;
+  int xs_ctas_per_sm;  // resident CTAs of xs_mul_kernel per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor)
 };
 
 // Kernel family of S*x, and with it of the Schur initialisation, J'J x and the evaluation.  Tile: the CTA-tile kernels
@@ -134,11 +136,12 @@ inline bool is_v4(MulFamily m) { return m == MulFamily::V4 || m == MulFamily::V4
 // Block pattern of the upper triangle of S and what its assembly and product read (explicit_schur.cuh), built from the
 // row structure in the internal order.  Block row i: the diagonal block first (also for a camera without rows), then
 // the cameras j > i sharing a point with i in increasing order; every block lists its row pairs (r, s) in the order
-// (row r of camera i in row order, row s of r's point in row order) -- a fixed summation order.
+// (row r of camera i in row order, row s of r's point in row order) -- a fixed summation order.  T slots: the
+// off-diagonal blocks ordered by column, then by row.
 struct XsPattern {
   long long off_blocks = 0;   // distinct camera pairs i < j that share a point
-  std::vector<int> blk_row, blk_col, pair_ptr, list_ptr;
-  std::vector<int2> pairs, list;
+  std::vector<int> blk_row, blk_col, pair_ptr, row_ptr, col_ptr;
+  std::vector<int2> pairs, cols;
 };
 
 struct KernelPlan {
@@ -179,8 +182,9 @@ struct KernelPlan {
   bool xs = false;
   XsPattern xp;
   std::vector<int> xs_order;           // [long blocks | short blocks]
-  std::vector<int> xs_warp_cam;
-  int num_xs_long = 0, xs_grid = 0;
+  std::vector<int2> xs_steps;         // product steps (XsView::steps), warp by warp
+  std::vector<int> xs_warp_step;
+  int num_xs_long = 0, xs_grid = 0, xs_resident = 0, xs_max_steps = 0;
   double bytes_per_op[K_COUNT] = {};
 };
 
@@ -193,7 +197,8 @@ inline void xs_pattern(int C, int N, const int* cam_idx, const int* pt_idx, cons
     for (int r = 0; r < N; ++r) crow[fill[cam_idx[r]]++] = r;
   }
   std::vector<int> stamp(static_cast<size_t>(C), -1), slot(static_cast<size_t>(C), 0), js, start;
-  std::vector<int> row_start(static_cast<size_t>(C) + 1, 0);
+  std::vector<int>& row_start = xp->row_ptr;
+  row_start.assign(static_cast<size_t>(C) + 1, 0);
   std::vector<int3> tup;
   for (int i = 0; i < C; ++i) {
     js.clear();
@@ -231,26 +236,15 @@ inline void xs_pattern(int C, int N, const int* cam_idx, const int* pt_idx, cons
   const int nb = static_cast<int>(xp->blk_row.size());
   row_start[C] = nb;
   xp->pair_ptr.push_back(static_cast<int>(xp->pairs.size()));
-  // product lists: block row i, then the blocks (j, i) above the diagonal of column i, in order of j
-  std::vector<int> tcnt(static_cast<size_t>(C) + 1, 0);
+  // T slots by column, each column's blocks in order of their row
+  xp->col_ptr.assign(static_cast<size_t>(C) + 1, 0);
   for (int b = 0; b < nb; ++b)
-    if (xp->blk_col[b] != xp->blk_row[b]) tcnt[xp->blk_col[b] + 1]++;
-  for (int c = 0; c < C; ++c) tcnt[c + 1] += tcnt[c];
-  std::vector<int2> tr(static_cast<size_t>(tcnt[C]));
-  {
-    std::vector<int> fill(tcnt.begin(), tcnt.end() - 1);
-    for (int b = 0; b < nb; ++b)
-      if (xp->blk_col[b] != xp->blk_row[b])
-        tr[fill[xp->blk_col[b]]++] = make_int2(b, static_cast<int>(static_cast<uint32_t>(xp->blk_row[b]) | kXsTransposed));
-  }
-  xp->list_ptr.assign(static_cast<size_t>(C) + 1, 0);
-  xp->list.reserve(static_cast<size_t>(nb) + tr.size());
-  for (int i = 0; i < C; ++i) {
-    xp->list_ptr[i] = static_cast<int>(xp->list.size());
-    for (int b = row_start[i]; b < row_start[i + 1]; ++b) xp->list.push_back(make_int2(b, xp->blk_col[b]));
-    xp->list.insert(xp->list.end(), tr.begin() + tcnt[i], tr.begin() + tcnt[i + 1]);
-  }
-  xp->list_ptr[C] = static_cast<int>(xp->list.size());
+    if (xp->blk_col[b] != xp->blk_row[b]) xp->col_ptr[xp->blk_col[b] + 1]++;
+  for (int c = 0; c < C; ++c) xp->col_ptr[c + 1] += xp->col_ptr[c];
+  std::vector<int> fill(xp->col_ptr.begin(), xp->col_ptr.end() - 1);
+  xp->cols.resize(static_cast<size_t>(nb));
+  for (int b = 0; b < nb; ++b)
+    xp->cols[b] = make_int2(xp->blk_col[b], xp->blk_col[b] != xp->blk_row[b] ? fill[xp->blk_col[b]]++ : -1);
 }
 
 // ---- Internal point order.  The fast kernels give every persistent CTA a contiguous run of points and keep the cameras
@@ -750,9 +744,12 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
     xs_pattern(C, N, cam_idx, pt_idx, pt_ptr.data(), &xp);
     const double nb = static_cast<double>(xp.blk_row.size()), npairs = static_cast<double>(xp.pairs.size());
     const double implicit_bytes = 196.0 * N + 52.0 * P + 216.0 * C;
-    xs_mul_bytes = 648.0 * xp.list.size() + 8.0 * xp.list.size() + 216.0 * C;   // blocks as listed (off-diagonal twice), list, x, y
+    const double off = static_cast<double>(xp.off_blocks);
+    const double two_pass_bytes = 656.0 * (nb + off) + 216.0 * C;   // the decision's yardstick (kXsByteRatio)
     const double storage = 648.0 * nb + 8.0 * npairs + 12.0 * nb;
-    pl.xs = implicit_bytes >= kXsByteRatio * xs_mul_bytes && implicit_bytes > l2_budget && storage <= kXsMaxBytes && npairs < 2.0e9;
+    pl.xs = implicit_bytes >= kXsByteRatio * two_pass_bytes && implicit_bytes > l2_budget && storage <= kXsMaxBytes && npairs < 2.0e9;
+    // S read once, its column entries, T written, x read, y written
+    xs_mul_bytes = 656.0 * nb + 72.0 * off + 144.0 * C;
     if (knobs.explicit_s >= 0) pl.xs = knobs.explicit_s != 0 && npairs < 2.0e9;
     // J, point of each row, (E'E+D^2)^-1, row pairs, block table; S and the diagonal upper triangles written
     xs_asm_bytes = 196.0 * N + 48.0 * P + 8.0 * npairs + 12.0 * nb + 648.0 * nb + 360.0 * C;
@@ -760,20 +757,30 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
   if (pl.xs) {
     const XsPattern& xp = pl.xp;
     const int nb = static_cast<int>(xp.blk_row.size());
-    // product warp groups: contiguous camera ranges balanced by list length (+ a per-camera overhead)
-    const int groups_want = std::max(1, std::min(C, 4 * lim.sm_count * kXsGroups));
-    pl.xs_grid = (groups_want + kXsGroups - 1) / kXsGroups;
-    const int nw = pl.xs_grid * kXsGroups;
-    pl.xs_warp_cam.assign(static_cast<size_t>(nw) + 1, C);   // warps past the last owner start (and end) at C
-    const double per_cam = 4.0;
-    const double total = static_cast<double>(xp.list.size()) + per_cam * C;
+    // One wave: at most the CTAs that are resident together, and no more warps than block rows.  Each warp owns a
+    // contiguous range of block rows, balanced by its steps (kXsStep blocks each) plus one per row for the row's sum.
+    pl.xs_resident = std::max(1, lim.xs_ctas_per_sm) * lim.sm_count;
+    pl.xs_grid = std::max(1, std::min(pl.xs_resident, (C + kXsWarps - 1) / kXsWarps));
+    const int nw = pl.xs_grid * kXsWarps;
+    auto row_steps = [&](int i) { return (xp.row_ptr[i + 1] - xp.row_ptr[i] + kXsStep - 1) / kXsStep; };
+    double total = 0.0;
+    for (int i = 0; i < C; ++i) total += row_steps(i) + 1;
+    pl.xs_warp_step.assign(static_cast<size_t>(nw) + 1, 0);
     double cum = 0.0;
     int w = 0;
     for (int i = 0; i < C; ++i) {
       const int owner = std::min(nw - 1, static_cast<int>(cum * nw / total));
-      while (w <= owner) pl.xs_warp_cam[w++] = i;
-      cum += (xp.list_ptr[i + 1] - xp.list_ptr[i]) + per_cam;
+      while (w < owner) pl.xs_warp_step[++w] = static_cast<int>(pl.xs_steps.size());   // warps before the owner end here
+      const int r0 = xp.row_ptr[i], r1 = xp.row_ptr[i + 1];
+      for (int b = r0; b < r1; b += kXsStep) {
+        const int n = std::min(kXsStep, r1 - b);
+        pl.xs_steps.push_back(make_int2(b, i | (n << kXsStepCountShift) | (b == r0 ? kXsStepFirst : 0) |
+                                               (b + kXsStep >= r1 ? kXsStepLast : 0)));
+      }
+      cum += row_steps(i) + 1;
     }
+    while (w < nw) pl.xs_warp_step[++w] = static_cast<int>(pl.xs_steps.size());
+    for (int k = 0; k < nw; ++k) pl.xs_max_steps = std::max(pl.xs_max_steps, pl.xs_warp_step[k + 1] - pl.xs_warp_step[k]);
     // the blocks with long pair lists (the diagonal ones, mostly) first, one CTA each; then one warp per block
     pl.xs_order.reserve(static_cast<size_t>(nb));
     for (int b = 0; b < nb; ++b)
@@ -831,10 +838,13 @@ inline void print_plan(const KernelPlan& pl, int C, int P, int N, int world, con
           C, P, N, pl.wtiles.size(), pl.big_tiles.size(), static_cast<int>(pl.huge_pts.size()), pl.max_cam_span, v.direct, v.warps, v.stages,
           v.replicas, mul_names[static_cast<int>(pl.mul)], m.warps, m.stages, m.replicas, pl.mul_smem, pl.big_folded ? 1 : 0,
           is_v4(pl.mul) ? 1 : 0, pl.diag == DiagPass::CamMajor ? 1 : 0, diag_names[static_cast<int>(pl.diag)]);
-  if (world == 1)
+  if (world == 1) {
     fprintf(stderr, "[b200ba] S plan: %s, %lld pairs, %.1f MB\n", pl.xs ? "explicit" : "implicit", pl.xp.off_blocks,
             648.0 * static_cast<double>(pl.xp.blk_row.size()) / 1e6);
-  else
+    if (pl.xs)
+      fprintf(stderr, "[b200ba] S product: grid %d of %d resident CTAs (%d per SM), %d warps, at most %d steps per warp\n",
+              pl.xs_grid, pl.xs_resident, lim.xs_ctas_per_sm, pl.xs_grid * kXsWarps, pl.xs_max_steps);
+  } else
     fprintf(stderr, "[b200ba] S plan: implicit, sharded\n");
 }
 
