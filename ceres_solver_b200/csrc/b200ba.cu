@@ -251,6 +251,10 @@ struct b200_handle {
   XsView xsv{};
   int num_xs_long = 0, num_xs_short = 0;   // blocks assembled by a CTA / by a warp each
   int* d_xs_order = nullptr;   // [long blocks | short blocks]
+  // resident PCG on explicit S (xs_pcg.cuh): one cooperative launch per SCHUR_JACOBI solve
+  bool xs_pcg = false;
+  XsPcgArgs xpa{};             // the plan's geometry and the device arrays; the solve fills in its options and vectors
+  size_t xs_pcg_smem = 0;
   double* d_red = nullptr;    // per-CTA partial sums of cg_vector_kernel
   // multi-GPU exchange of the per-iteration partial products over NVLink peer memory (cg_kernel.cuh: xchg_push_kernel +
   // the gather in cg_vector_kernel); replaces the ncclAllReduce inside the PCG iteration when every peer could be mapped
@@ -857,6 +861,41 @@ int schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, const 
     OK(pcg_general_dev(h, o));
     return finish();
   }
+  if (explicit_s && h->xs_pcg) {
+    // the whole solve in one cooperative launch with S in shared memory (xs_pcg.cuh): no batches, no polling
+    if (!h->xs_ready) OK(xs_assemble_dev(h));
+    XsPcgArgs a = h->xpa;
+    a.prm = prm;
+    a.reset = o->residual_reset_period > 0 ? o->residual_reset_period : std::numeric_limits<int>::max();
+    a.minv = h->d_minv;
+    a.rhs = h->d_rhs;
+    a.Df = Df;
+    a.x = h->d_sol;
+    a.z = h->d_z;
+    a.p[0] = h->d_p;
+    a.st = h->d_cg;
+    void* args[] = {&a};
+    OK(launch(h, K_SCHUR_PCG, [&] {
+      cudaLaunchCooperativeKernel(reinterpret_cast<void*>(xs_pcg_kernel), dim3(h->sm_count), dim3(kXpThreads), args, h->xs_pcg_smem,
+                                  h->stream);
+    }));
+    CU(cudaMemcpyAsync(h->h_cg, h->d_cg, sizeof(CgState), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    // operations: the products of the solve, one per iteration that reached it (a failed rho / beta check counts the
+    // iteration it could not start) and one per residual reset
+    const CgState& s = *h->h_cg;
+    const int its = std::max(0, s.iteration - (s.reason == 4 || s.reason == 5 ? 1 : 0));
+    h->ops[K_SCHUR_PCG] += its + its / a.reset - 1;   // launch() counted one
+#ifdef B200_DEV_KNOBS
+    if (a.stamps != nullptr) {
+      long long t[kXpPhases];
+      CU(cudaMemcpy(t, a.stamps, sizeof(t), cudaMemcpyDeviceToHost));
+      fprintf(stderr, "[b200ba] xs_pcg stamps (CTA 0, cycles, cumulative): begin %lld product %lld barrier1 %lld vector %lld barrier2 %lld tests %lld\n",
+              t[0], t[1], t[2], t[3], t[4], t[5]);
+    }
+#endif
+    return finish();
+  }
   OK(vec(CG_BEGIN, h->d_z, h->d_z));
   const int reset = o->residual_reset_period > 0 ? o->residual_reset_period : std::numeric_limits<int>::max();
   // Termination is decided on the device; the host only polls the state every few iterations (kernels become
@@ -1214,6 +1253,7 @@ int set_func_attributes(int smem_optin) {
   OK(raise_smem_limit(evaluate_v2_kernel<false>, lim));
   OK(raise_smem_limit(diag_blocks_v2_kernel<true>, lim));
   OK(raise_smem_limit(diag_blocks_v2_kernel<false>, lim));
+  OK(raise_smem_limit(xs_pcg_kernel, lim));
   return B200_OK;
 }
 
@@ -1317,7 +1357,10 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   CU(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, desc->device));
   int xs_per_sm = 0;   // the explicit-S product's grid is one wave of these (plan.cuh)
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&xs_per_sm, xs_mul_kernel, kXsThreads, 0));
-  const DevLimits lim{prop.multiProcessorCount, prop.sharedMemPerBlockOptin, l2_bytes, xs_per_sm};
+  int xs_pcg_per_sm = 0;   // the resident PCG needs one CTA per SM at the most shared memory it may plan
+  OK(set_func_attributes(static_cast<int>(prop.sharedMemPerBlockOptin)));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&xs_pcg_per_sm, xs_pcg_kernel, kXpThreads, prop.sharedMemPerBlockOptin - 1024));
+  const DevLimits lim{prop.multiProcessorCount, prop.sharedMemPerBlockOptin, l2_bytes, xs_per_sm, xs_pcg_per_sm};
   const DevKnobs knobs = DevKnobs::from_env();
   const int world = desc->world_size > 1 ? desc->world_size : 1;
   KernelPlan pl;
@@ -1476,9 +1519,27 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     h->num_xs_long = pl.num_xs_long;
     h->num_xs_short = x.num_blocks - pl.num_xs_long;
     h->xs_grid = pl.xs_grid;
+    h->xs_pcg = pl.xs_pcg;
+    if (h->xs_pcg) {
+      XsPcgArgs& a = h->xpa;
+      a.v = x;
+      OK(upload(h, pl.xs_pcg_cta, &a.cta));
+      OK(upload(h, pl.xs_pcg_warp_step, &a.warp_step));
+      a.max_blocks = pl.xs_pcg_max_blocks;
+      a.max_cams = pl.xs_pcg_max_cams;
+      OK(dev_alloc(h, &a.p[1], nc));   // the second p buffer; the first is d_p
+      OK(dev_alloc(h, &a.red, static_cast<size_t>(prop.multiProcessorCount) * 4));
+      h->xs_pcg_smem = pl.xs_pcg_smem;
+#ifdef B200_DEV_KNOBS
+      a.stamps = nullptr;
+      if (dev_env("B200_XS_STAMPS") != nullptr) {
+        OK(dev_alloc(h, &a.stamps, kXpPhases));
+        CU(cudaMemsetAsync(a.stamps, 0, sizeof(long long) * kXpPhases, h->stream));
+      }
+#endif
+    }
   }
   CU(cudaStreamSynchronize(h->stream));
-  OK(set_func_attributes(static_cast<int>(prop.sharedMemPerBlockOptin)));
 
   for (int k = 0; k < K_COUNT; ++k) h->grid_tile[k] = std::max(1, std::min(h->num_tiles, h->sm_count * 4));
   h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<true>, tile_smem_bytes<3, 1>());

@@ -94,7 +94,8 @@ struct CgVecArgs {
   unsigned xg_epoch;
 };
 
-// Sums up to three values over the CTA with one barrier pair; results valid in every thread.
+// Sums up to three values over a CTA of kWarps warps with one barrier pair; results valid in every thread.
+template <int kWarps = kCgThreads / 32>
 __device__ __forceinline__ void cg_block_sum3(double& a, double& b, double& c, double (*scratch)[3]) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -112,7 +113,7 @@ __device__ __forceinline__ void cg_block_sum3(double& a, double& b, double& c, d
   __syncthreads();
   a = b = c = 0.0;
 #pragma unroll
-  for (int w = 0; w < kCgThreads / 32; ++w) {
+  for (int w = 0; w < kWarps; ++w) {
     a += scratch[w][0];
     b += scratch[w][1];
     c += scratch[w][2];
@@ -133,6 +134,118 @@ __device__ __forceinline__ void cg_totals(const double* red, int nb, int slot0, 
   __syncthreads();
   for (int k = 0; k < count; ++k) out[k] = s_tot[k];
 }
+
+// The reference's tests of one PCG iteration (conjugate_gradients_solver.h:162-299), shared by cg_vector_kernel and the
+// resident PCG (xs_pcg.cuh).  Every CTA evaluates them on identical totals, so every CTA takes the same branch; `writer`
+// (one thread of the grid) publishes the state the host reads.
+//
+// p.q of iteration `it`: false when the solve stops here, else alpha = rho_old / p.q.
+__device__ __forceinline__ bool cg_alpha(double pq, double rho_old, int it, CgState* st, bool writer, double* alpha) {
+  int term = 0, reason = 0;
+  if (!(pq > 0.0) || isinf(pq)) {
+    term = isnan(pq) ? 2 : 1;
+    reason = 6;
+  } else {
+    *alpha = rho_old / pq;
+    if (!isinf(*alpha)) return true;
+    term = 2;
+    reason = 7;
+  }
+  if (writer) {
+    st->pq = pq;
+    st->done = 1;
+    st->termination = term;
+    st->reason = reason;
+    st->iteration = it;
+  }
+  return false;
+}
+
+// Phase C: the termination tests of iteration `it` (or, `begin`, of the initial residual) on the totals x.(b+r), r.r and
+// r.z, then the rho / beta checks of iteration it + 1.  False when the solve ends here; otherwise beta (0 for it == 0),
+// the Q0 and |r| tolerance the next iteration tests against, and the state of the next iteration published.
+__device__ __forceinline__ bool cg_phase_c(const CgParams& prm, bool begin, int it, double rho_old, double Q0, double tol_r,
+                                           double dotQ, double sqR, double rho_new, CgState* st, bool writer, double* beta,
+                                           double* Q0_next, double* tol_r_next) {
+  const double norm_r = sqrt(sqR);
+  *Q0_next = 0.0;
+  *tol_r_next = tol_r;
+  if (begin) {
+    if (writer) {
+      st->norm_rhs = norm_r;
+      st->tol_r = prm.r_tolerance * norm_r;
+      st->norm_r = norm_r;
+      st->Q0 = 0.0;
+      st->iteration = 0;
+      st->done = 0;
+      st->termination = 1;
+      st->reason = 0;
+      st->last_rho = 1.0;
+    }
+    const double tol0 = prm.r_tolerance * norm_r;
+    *tol_r_next = tol0;
+    if (norm_r == 0.0 || (prm.min_iterations == 0 && norm_r <= tol0)) {
+      if (writer) {
+        st->done = 1;
+        st->termination = 0;
+        st->reason = norm_r == 0.0 ? 8 : 2;
+      }
+      return false;
+    }
+  } else {
+    // termination tests of iteration `it`
+    const double Q1 = -dotQ;
+    const double zeta = it * (Q1 - Q0) / Q1;
+    int done = 0, term = 1, reason = 0;
+    if (zeta < prm.q_tolerance && it >= prm.min_iterations) {
+      done = 1; term = 0; reason = 1;
+    } else if (norm_r <= tol_r && it >= prm.min_iterations) {
+      done = 1; term = 0; reason = 2;
+    } else if (it >= prm.max_iterations) {
+      done = 1; term = 1; reason = 3;
+    }
+    if (done) {
+      if (writer) {
+        st->norm_r = norm_r;
+        st->iteration = it;
+        st->done = 1;
+        st->termination = term;
+        st->reason = reason;
+      }
+      return false;
+    }
+    *Q0_next = Q1;
+  }
+  // rho / beta checks of iteration it + 1
+  *beta = 0.0;
+  int fail_reason = 0;
+  if (zero_or_inf(rho_new) || isnan(rho_new)) {
+    fail_reason = 4;
+  } else if (it >= 1) {
+    *beta = rho_new / rho_old;
+    if (zero_or_inf(*beta)) fail_reason = 5;
+  }
+  if (fail_reason) {
+    if (writer) {
+      st->iteration = it + 1;
+      st->done = 1;
+      st->termination = 2;
+      st->reason = fail_reason;
+    }
+    return false;
+  }
+  if (writer) {
+    st->norm_r = norm_r;
+    st->last_rho = rho_old;
+    st->rho = rho_new;
+    st->Q0 = *Q0_next;
+    st->iteration = it;
+  }
+  return true;
+}
+
+// The next search direction p = z + beta p (p = z in the first iteration), one expression for every kernel that forms it.
+__device__ __forceinline__ double cg_next_p(int it, double z, double beta, double p) { return it == 0 ? z : __fma_rn(beta, p, z); }
 
 __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
   cg::grid_group grid = cg::this_grid();
@@ -257,30 +370,7 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
     } else {
       cg_totals(a.red, gridDim.x, 0, 1, &pq, s_tot);
     }
-    bool stop = false;
-    int term = 0, reason = 0;
-    if (!(pq > 0.0) || isinf(pq)) {
-      stop = true;
-      term = isnan(pq) ? 2 : 1;
-      reason = 6;
-    } else {
-      alpha = rho_old / pq;
-      if (isinf(alpha)) {
-        stop = true;
-        term = 2;
-        reason = 7;
-      }
-    }
-    if (stop) {
-      if (writer) {
-        st->pq = pq;
-        st->done = 1;
-        st->termination = term;
-        st->reason = reason;
-        st->iteration = it;
-      }
-      return;  // every CTA takes this branch together
-    }
+    if (!cg_alpha(pq, rho_old, it, st, writer, &alpha)) return;  // every CTA takes this branch together
   }
   double zj = 0.0;
   {
@@ -361,78 +451,15 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
   // ------------------------------------------------------------------ phase C
   double tot[3];
   cg_totals(a.red, gridDim.x, 1, 3, tot, s_tot);
-  const double dotQ = tot[0], sqR = tot[1], rho_new = tot[2];
-  const double norm_r = sqrt(sqR);
-  double Q0_next = 0.0;
-  if (mode == CG_BEGIN) {
-    if (writer) {
-      st->norm_rhs = norm_r;
-      st->tol_r = a.prm.r_tolerance * norm_r;
-      st->norm_r = norm_r;
-      st->Q0 = 0.0;
-      st->iteration = 0;
-      st->done = 0;
-      st->termination = 1;
-      st->reason = 0;
-      st->last_rho = 1.0;
-    }
-    const double tol0 = a.prm.r_tolerance * norm_r;
-    if (norm_r == 0.0 || (a.prm.min_iterations == 0 && norm_r <= tol0)) {
-      if (writer) {
-        st->done = 1;
-        st->termination = 0;
-        st->reason = norm_r == 0.0 ? 8 : 2;
-      }
-      return;
-    }
-  } else {
-    // termination tests of iteration `it`
-    const double Q1 = -dotQ;
-    const double zeta = it * (Q1 - Q0) / Q1;
-    int done = 0, term = 1, reason = 0;
-    if (zeta < a.prm.q_tolerance && it >= a.prm.min_iterations) {
-      done = 1; term = 0; reason = 1;
-    } else if (norm_r <= tol_r && it >= a.prm.min_iterations) {
-      done = 1; term = 0; reason = 2;
-    } else if (it >= a.prm.max_iterations) {
-      done = 1; term = 1; reason = 3;
-    }
-    if (done) {
-      if (writer) {
-        st->norm_r = norm_r;
-        st->iteration = it;
-        st->done = 1;
-        st->termination = term;
-        st->reason = reason;
-      }
-      return;
-    }
-    Q0_next = Q1;
-  }
-  // rho / beta checks of iteration it + 1, then p
-  double beta = 0.0;
-  {
-    int fail_reason = 0;
-    if (zero_or_inf(rho_new) || isnan(rho_new)) {
-      fail_reason = 4;
-    } else if (it >= 1) {
-      beta = rho_new / rho_old;
-      if (zero_or_inf(beta)) fail_reason = 5;
-    }
-    if (fail_reason) {
-      if (writer) {
-        st->iteration = it + 1;
-        st->done = 1;
-        st->termination = 2;
-        st->reason = fail_reason;
-      }
-      return;
-    }
-  }
+  // termination tests, then the rho / beta checks of iteration it + 1 and the state of the next launch; then p
+  double beta = 0.0, Q0_next = 0.0, tol_next = 0.0;
+  if (!cg_phase_c(a.prm, mode == CG_BEGIN, it, rho_old, Q0, tol_r, tot[0], tot[1], tot[2], st, writer, &beta, &Q0_next,
+                  &tol_next))
+    return;
   double seed_acc = 0.0;
   if (single) {
     if (ok0) {
-      const double pn = (it == 0) ? zj : zj + beta * pj;
+      const double pn = cg_next_p(it, zj, beta, pj);
       a.p[j0] = pn;
       if (a.seed_target != nullptr) a.seed_target[j0] = dj * dj * pn;
       seed_acc = dj * dj * pn * pn;
@@ -441,7 +468,7 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
     for (int blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
       const int j = blk * kCgCamsPerCta * 9 + tid;
       if (lane_ok && j < n) {
-        const double pn = (it == 0) ? a.z[j] : a.z[j] + beta * a.p[j];
+        const double pn = cg_next_p(it, a.z[j], beta, a.p[j]);
         a.p[j] = pn;
         const double d = a.Df != nullptr ? a.Df[j] : 0.0;
         if (a.seed_target != nullptr) a.seed_target[j] = d * d * pn;
@@ -453,13 +480,6 @@ __global__ void __launch_bounds__(kCgThreads) cg_vector_kernel(CgVecArgs a) {
     double d1 = 0.0, d2 = 0.0;
     cg_block_sum3(seed_acc, d1, d2, scratch);
     if (tid == 0) a.seed_pq[blockIdx.x] = seed_acc;
-  }
-  if (writer) {
-    st->norm_r = norm_r;
-    st->last_rho = rho_old;
-    st->rho = rho_new;
-    st->Q0 = Q0_next;
-    st->iteration = it;
   }
 }
 

@@ -18,8 +18,8 @@
 // Product (one pass over the stored triangle).  The warp that owns block row i streams it once, three blocks per step
 // (lane 9e + w holds column w of the step's block e, lanes 27..31 idle).  For each block (i, j) it adds S_ij x_j into
 // the row part a_i, and for j > i it also forms t_ij = S_ij' x_i, which it stores in the block's slot of T.  It writes
-// y_i = seed + a_i; the column part sum_{i<j} t_ij of q_j is added by whoever reads q next: the PCG's vector kernel
-// (xs_col_sum) or, outside the PCG, xs_gather_kernel.  T is ordered by column, so that sum reads contiguous slots.
+// y_i = seed + a_i; the column part sum_{i<j} t_ij of q_j is added by whoever reads q next: the PCG's vector kernel or
+// the vector phase of the resident PCG (xs_col_sum, xs_pcg.cuh) or, outside the PCG, xs_gather_kernel.  T is ordered by column, so that sum reads contiguous slots.
 #pragma once
 #include "common.cuh"
 
@@ -186,28 +186,30 @@ __device__ __forceinline__ void xs_step_s(const XsView& v, int2 d, int e, int w,
   for (int u = 0; u < 9; ++u) s[u] = in ? __ldg(sb + 9 * u) : 0.0;
 }
 
-// y = [y if accumulate] + [D_f^2 x if Df] + (row part of S x), and T = the column part (file comment), S as assembled
-// (without D_f^2).  Inside the PCG: accumulate onto the output the vector kernel seeded, no-op once done_flag is set, and
-// pq_part[CTA] = sum over this CTA's rows of x_i . a_i + sum over its off-diagonal blocks of x_j . t_ij, i.e. its share of
-// x . S x -- the product protocol of schur_mul_v4_kernel.  Launched with programmatic stream serialisation behind the
-// vector kernel: the steps, column entries and S of the first two steps are static and are read before the wait.
-// Each warp walks its steps with the next step's S and x_j in flight and the column entries of the one after.
-__global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v, const double* __restrict__ x, double* y,
-                                                                        const double* __restrict__ Df, int accumulate,
-                                                                        const int* __restrict__ done_flag, double* pq_part) {
-  __shared__ double s_pq[kXsWarps];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int e = lane / 9, w = lane - 9 * (lane / 9);   // e == 3: lanes 27..31, no block
-  const int gw = blockIdx.x * kXsWarps + warp;
-  const int k0 = __ldg(v.warp_step + gw), k1 = __ldg(v.warp_step + gw + 1);
+// The walk of one warp over its product steps [k0, k1), shared by xs_mul_kernel and the resident PCG (xs_pcg.cuh), so that
+// both form S x with the same arithmetic in the same order: lane 9e + w, the next step's S and x_j in flight and the
+// column entries of the one after, the butterfly of each row sum, and t_ij stored into its T slot.  load_s(d, e, w, s)
+// fills the lane's column of step d's block e, load_x(j, w) returns entry w of x_j, row_out(i, lane, a_i[lane], x_i[lane])
+// takes the row part of row i in lanes 0..8.  xs_walk_begin loads what does not depend on x (before a grid dependency
+// resolves); xs_walk returns the lane's share of x . S x (x_i . a_i over its rows, x_j . t_ij over its blocks).
+struct XsWalk {
   XsStepData nx;   // step k + 1
-  nx.d = xs_step_desc(v, k0, k1);
-  nx.c = xs_step_col(v, nx.d, e);
-  xs_step_s(v, nx.d, e, w, nx.s);
-  int2 d2 = xs_step_desc(v, k0 + 1, k1), c2 = xs_step_col(v, d2, e);   // step k + 2: descriptor and column entry
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  if (done_flag != nullptr && __ldcg(done_flag) != 0) return;
-  double nx_x = xs_lane_in(nx.d, e) ? __ldcg(x + 9 * static_cast<size_t>(nx.c.x) + w) : 0.0;
+  int2 d2, c2;     // step k + 2: descriptor and column entry
+};
+template <class LoadS>
+__device__ __forceinline__ void xs_walk_begin(const XsView& v, int k0, int k1, int e, int w, LoadS load_s, XsWalk& wk) {
+  wk.nx.d = xs_step_desc(v, k0, k1);
+  wk.nx.c = xs_step_col(v, wk.nx.d, e);
+  load_s(wk.nx.d, e, w, wk.nx.s);
+  wk.d2 = xs_step_desc(v, k0 + 1, k1);
+  wk.c2 = xs_step_col(v, wk.d2, e);
+}
+template <class LoadS, class LoadX, class RowOut>
+__device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int lane, int e, int w, LoadS load_s, LoadX load_x,
+                                          RowOut row_out, XsWalk& wk) {
+  XsStepData& nx = wk.nx;
+  int2 d2 = wk.d2, c2 = wk.c2;
+  double nx_x = xs_lane_in(nx.d, e) ? load_x(nx.c.x, w) : 0.0;
   double acc[9], xi[9];
 #pragma unroll
   for (int u = 0; u < 9; ++u) acc[u] = xi[u] = 0.0;
@@ -221,8 +223,8 @@ __global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v
     // refill: step k + 1 from the entries loaded one step ago, the column entries of step k + 2
     nx.d = d2;
     nx.c = c2;
-    xs_step_s(v, nx.d, e, w, nx.s);
-    nx_x = xs_lane_in(nx.d, e) ? __ldcg(x + 9 * static_cast<size_t>(nx.c.x) + w) : 0.0;
+    load_s(nx.d, e, w, nx.s);
+    nx_x = xs_lane_in(nx.d, e) ? load_x(nx.c.x, w) : 0.0;
     d2 = xs_step_desc(v, k + 2, k1);
     c2 = xs_step_col(v, d2, e);
     // a row begins with its diagonal block in lanes 0..8: their x_j is x_i
@@ -254,15 +256,42 @@ __global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v
         acc[u] = 0.0;
       }
       if (lane < 9) {
-        const size_t o = 9 * static_cast<size_t>(d.y & ((1 << kXsStepCountShift) - 1)) + lane;
         pq += xo * mine;
-        double out = mine;
-        if (Df != nullptr) out += Df[o] * Df[o] * xo;
-        if (accumulate) out += __ldcg(y + o);
-        y[o] = out;
+        row_out(d.y & ((1 << kXsStepCountShift) - 1), lane, mine, xo);
       }
     }
   }
+  return pq;
+}
+
+// y = [y if accumulate] + [D_f^2 x if Df] + (row part of S x), and T = the column part (file comment), S as assembled
+// (without D_f^2).  Inside the PCG: accumulate onto the output the vector kernel seeded, no-op once done_flag is set, and
+// pq_part[CTA] = sum over this CTA's rows of x_i . a_i + sum over its off-diagonal blocks of x_j . t_ij, i.e. its share of
+// x . S x -- the product protocol of schur_mul_v4_kernel.  Launched with programmatic stream serialisation behind the
+// vector kernel: the steps, column entries and S of the first two steps are static and are read before the wait.
+__global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v, const double* __restrict__ x, double* y,
+                                                                        const double* __restrict__ Df, int accumulate,
+                                                                        const int* __restrict__ done_flag, double* pq_part) {
+  __shared__ double s_pq[kXsWarps];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int e = lane / 9, w = lane - 9 * (lane / 9);   // e == 3: lanes 27..31, no block
+  const int gw = blockIdx.x * kXsWarps + warp;
+  const int k0 = __ldg(v.warp_step + gw), k1 = __ldg(v.warp_step + gw + 1);
+  auto load_s = [&](int2 d, int e, int w, double* s) { xs_step_s(v, d, e, w, s); };
+  XsWalk wk;
+  xs_walk_begin(v, k0, k1, e, w, load_s, wk);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (done_flag != nullptr && __ldcg(done_flag) != 0) return;
+  double pq = xs_walk(
+      v, k0, k1, lane, e, w, load_s, [&](int j, int w) { return __ldcg(x + 9 * static_cast<size_t>(j) + w); },
+      [&](int i, int u, double a, double xo) {
+        const size_t o = 9 * static_cast<size_t>(i) + u;
+        double out = a;
+        if (Df != nullptr) out += Df[o] * Df[o] * xo;
+        if (accumulate) out += __ldcg(y + o);
+        y[o] = out;
+      },
+      wk);
   if (pq_part == nullptr) return;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) pq += __shfl_xor_sync(0xffffffffu, pq, o);

@@ -15,6 +15,7 @@
 
 #include "explicit_schur.cuh"
 #include "kernels_v4b.cuh"
+#include "xs_pcg.cuh"
 
 namespace b200 {
 
@@ -53,13 +54,14 @@ enum KernelId {
   K_PMV_RIGHT_F,
   K_PMV_LEFT_E,
   K_PMV_LEFT_F,
+  K_SCHUR_PCG,
   K_MISC,
   K_COUNT
 };
 const char* const kKernelNames[K_COUNT] = {"evaluate_jacobian", "evaluate_cost", "squared_column_norm", "scale_columns",
                                            "jacobian_multiply", "jacobian_t_multiply", "jtj_multiply", "schur_init",
                                            "schur_multiply", "schur_multiply_big_points", "camera_reduce", "schur_diag_blocks", "invert_9x9", "back_substitute",
-                                           "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "misc"};
+                                           "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg", "misc"};
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.
@@ -88,6 +90,7 @@ struct DevKnobs {
   bool no_pdl = false;               // B200_NO_PDL
   bool no_fused_pq = false;          // B200_NO_FUSED_PQ
   bool no_peer_exchange = false;     // B200_NO_PEER_EXCHANGE
+  int xs_resident = -1;              // B200_XS_RESIDENT (-1: as planned; 0: the two-kernel explicit-S PCG)
 
   static DevKnobs from_env() {
     DevKnobs k;
@@ -111,6 +114,7 @@ struct DevKnobs {
     k.no_pdl = dev_env("B200_NO_PDL") != nullptr;
     k.no_fused_pq = dev_env("B200_NO_FUSED_PQ") != nullptr;
     k.no_peer_exchange = dev_env("B200_NO_PEER_EXCHANGE") != nullptr;
+    if (const char* e = dev_env("B200_XS_RESIDENT")) k.xs_resident = atoi(e) != 0 ? 1 : 0;
     return k;
   }
 };
@@ -120,6 +124,7 @@ struct DevLimits {
   size_t smem_optin;   // cudaDeviceProp::sharedMemPerBlockOptin
   int l2_bytes;
   int xs_ctas_per_sm;  // resident CTAs of xs_mul_kernel per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor)
+  int xs_pcg_ctas_per_sm;  // ... of xs_pcg_kernel with the most dynamic shared memory a CTA may take
 };
 
 // Kernel family of S*x, and with it of the Schur initialisation, J'J x and the evaluation.  Tile: the CTA-tile kernels
@@ -185,6 +190,13 @@ struct KernelPlan {
   std::vector<int2> xs_steps;         // product steps (XsView::steps), warp by warp
   std::vector<int> xs_warp_step;
   int num_xs_long = 0, xs_grid = 0, xs_resident = 0, xs_max_steps = 0;
+  // resident PCG on explicit S (xs_pcg.cuh): one CTA per SM, its block rows, their steps over its warps
+  bool xs_pcg = false;
+  std::vector<int2> xs_pcg_cta;        // [sm_count + 1] {first block row, first block}
+  std::vector<int> xs_pcg_warp_step;   // [sm_count * kXpWarps + 1] first step of each warp (into xs_steps)
+  int xs_pcg_max_blocks = 0, xs_pcg_max_cams = 0, xs_pcg_max_steps = 0;
+  size_t xs_pcg_smem = 0;
+  const char* xs_pcg_why = "";         // why the PCG is not resident
   double bytes_per_op[K_COUNT] = {};
 };
 
@@ -781,6 +793,68 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
     }
     while (w < nw) pl.xs_warp_step[++w] = static_cast<int>(pl.xs_steps.size());
     for (int k = 0; k < nw; ++k) pl.xs_max_steps = std::max(pl.xs_max_steps, pl.xs_warp_step[k + 1] - pl.xs_warp_step[k]);
+    // Resident PCG (xs_pcg.cuh): the block rows in G contiguous ranges with the smallest possible largest range in blocks
+    // (the share of S a CTA holds in shared memory): the least capacity K at which filling the CTAs in row order, each up
+    // to K blocks, needs at most G of them.  Within a CTA its rows go to the warps balanced by steps plus one per row, as
+    // above.  Resident when the largest CTA's blocks, M^-1 blocks and vectors fit one CTA's shared memory next to the
+    // static scratch, and one CTA of the kernel fits each SM.
+    {
+      const int G = lim.sm_count;
+      std::vector<int> first_step(static_cast<size_t>(C) + 1, 0);
+      for (int i = 0; i < C; ++i) first_step[i + 1] = first_step[i] + row_steps(i);
+      auto row_blocks = [&](int i) { return xp.row_ptr[i + 1] - xp.row_ptr[i]; };
+      auto ctas_at = [&](int K) {
+        int g = 1, cur = 0;
+        for (int i = 0; i < C; ++i) {
+          if (cur + row_blocks(i) > K) {
+            ++g;
+            cur = 0;
+          }
+          cur += row_blocks(i);
+        }
+        return g;
+      };
+      int lo = (nb + G - 1) / G, hi = nb;
+      for (int i = 0; i < C; ++i) lo = std::max(lo, row_blocks(i));
+      while (lo < hi) {
+        const int mid = lo + (hi - lo) / 2;
+        if (ctas_at(mid) <= G) hi = mid;
+        else lo = mid + 1;
+      }
+      pl.xs_pcg_cta.assign(static_cast<size_t>(G) + 1, make_int2(C, nb));
+      pl.xs_pcg_cta[0] = make_int2(0, 0);
+      for (int i = 0, g = 0, cur = 0; i < C; ++i) {
+        if (cur + row_blocks(i) > lo) {
+          pl.xs_pcg_cta[++g] = make_int2(i, xp.row_ptr[i]);
+          cur = 0;
+        }
+        cur += row_blocks(i);
+      }
+      pl.xs_pcg_warp_step.assign(static_cast<size_t>(G) * kXpWarps + 1, first_step[C]);
+      for (int b = 0; b < G; ++b) {
+        const int i0 = pl.xs_pcg_cta[b].x, i1 = pl.xs_pcg_cta[b + 1].x;
+        pl.xs_pcg_max_blocks = std::max(pl.xs_pcg_max_blocks, pl.xs_pcg_cta[b + 1].y - pl.xs_pcg_cta[b].y);
+        pl.xs_pcg_max_cams = std::max(pl.xs_pcg_max_cams, i1 - i0);
+        double tot = 0.0, cum = 0.0;
+        for (int i = i0; i < i1; ++i) tot += row_steps(i) + 1;
+        int* ws = pl.xs_pcg_warp_step.data() + static_cast<size_t>(b) * kXpWarps;
+        int wv = 0;
+        ws[0] = first_step[i0];
+        for (int i = i0; i < i1; ++i) {
+          const int owner = std::min(kXpWarps - 1, static_cast<int>(cum * kXpWarps / tot));
+          while (wv < owner) ws[++wv] = first_step[i];
+          cum += row_steps(i) + 1;
+        }
+        while (wv < kXpWarps - 1) ws[++wv] = first_step[i1];
+      }
+      for (int k = 0; k < G * kXpWarps; ++k)
+        pl.xs_pcg_max_steps = std::max(pl.xs_pcg_max_steps, pl.xs_pcg_warp_step[k + 1] - pl.xs_pcg_warp_step[k]);
+      pl.xs_pcg_smem = xs_pcg_smem_bytes(pl.xs_pcg_max_blocks, pl.xs_pcg_max_cams);
+      if (pl.xs_pcg_smem + 1024 > lim.smem_optin) pl.xs_pcg_why = "largest CTA's shared memory exceeds the limit";
+      else if (lim.xs_pcg_ctas_per_sm < 1) pl.xs_pcg_why = "no CTA of the kernel fits an SM";
+      else if (knobs.xs_resident == 0) pl.xs_pcg_why = "B200_XS_RESIDENT=0";
+      else pl.xs_pcg = true;
+    }
     // the blocks with long pair lists (the diagonal ones, mostly) first, one CTA each; then one warp per block
     pl.xs_order.reserve(static_cast<size_t>(nb));
     for (int b = 0; b < nb; ++b)
@@ -813,6 +887,10 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
   if (pl.xs) {   // explicit S: the product and the assembly that replaces the block-diagonal pass
     bpo[K_SCHUR_MUL] = xs_mul_bytes;
     bpo[K_DIAG_BLOCKS] = xs_asm_bytes;
+    // one iteration of the resident PCG (xs_pcg.cuh): S and its column entries, T written and read, M^-1, and p, x, r, z
+    // read and written
+    const double nb = static_cast<double>(pl.xp.blk_row.size()), off = static_cast<double>(pl.xp.off_blocks);
+    if (pl.xs_pcg) bpo[K_SCHUR_PCG] = 656.0 * nb + 144.0 * off + 648.0 * Cc + 8 * 72.0 * Cc;
   }
 }
 
@@ -844,6 +922,16 @@ inline void print_plan(const KernelPlan& pl, int C, int P, int N, int world, con
     if (pl.xs)
       fprintf(stderr, "[b200ba] S product: grid %d of %d resident CTAs (%d per SM), %d warps, at most %d steps per warp\n",
               pl.xs_grid, pl.xs_resident, lim.xs_ctas_per_sm, pl.xs_grid * kXsWarps, pl.xs_max_steps);
+    if (pl.xs) {
+      const double share = 648.0 * pl.xs_pcg_max_blocks / 1024.0, limit = static_cast<double>(lim.smem_optin) / 1024.0;
+      const double cta = static_cast<double>(pl.xs_pcg_smem) / 1024.0;
+      if (pl.xs_pcg)
+        fprintf(stderr, "[b200ba] S PCG: resident, %d CTAs, largest S share %.2f KiB of %.2f KiB (%.2f KiB with M^-1 and vectors), %d warps, at most %d steps per warp\n",
+                lim.sm_count, share, limit, cta, lim.sm_count * kXpWarps, pl.xs_pcg_max_steps);
+      else
+        fprintf(stderr, "[b200ba] S PCG: two-kernel (%s: largest S share %.2f KiB, %.2f KiB with M^-1 and vectors, of %.2f KiB)\n",
+                pl.xs_pcg_why, share, cta, limit);
+    }
   } else
     fprintf(stderr, "[b200ba] S plan: implicit, sharded\n");
 }

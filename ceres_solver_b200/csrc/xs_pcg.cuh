@@ -1,0 +1,243 @@
+// The whole SCHUR_JACOBI PCG on an explicit S in one cooperative launch (DESIGN §3.2), for an S that fits the aggregate
+// shared memory of the SMs.  One CTA per SM owns a contiguous range of block rows -- the cameras of those rows and their
+// stored blocks -- and copies its blocks of S and its cameras' preconditioner blocks M^-1 into shared memory once per
+// solve.  Each iteration is then
+//   product  S p with S from shared memory (xs_walk, the arithmetic of xs_mul_kernel): the row part a_i of every owned
+//            camera stays in shared memory, t_ij goes to T, and the CTA's share of p.q (plus sum D_f^2 p^2) to red[.][0]
+//   ---- grid barrier ----
+//   vector   on the owned cameras: q = (a + D_f^2 p) + the column part from T (xs_col_sum), p.q, alpha, x, r, z = M^-1 r,
+//            and the partials of x.(b+r), r.r, r.z
+//   ---- grid barrier ----
+//   tests    the reference's termination and failure tests (cg_alpha, cg_phase_c) on identical fixed-order totals in
+//            every CTA, beta, and the new p of the owned cameras.
+// The product reads p_j of every column j its blocks touch.  A foreign column's p_j is not read back from its owner (that
+// would need a third barrier): the CTA forms it itself from z_j and the previous p_j (cg_next_p, the owner's expression,
+// so the bits agree).  p is double-buffered by iteration parity for that.  A residual reset adds a barrier, the product on
+// x and a second barrier, as CG_RESET_FIRST / CG_RESET_SECOND of the two-kernel loop do.  Every branch around a barrier
+// is taken by the whole grid: it depends only on the iteration count and on totals every CTA sums in the same order.
+// Everything another CTA wrote during the launch (z, p, x, T, red) is read with ld.global.cg.  No atomics: the solve is
+// deterministic given its inputs, and S q equals xs_mul_kernel + xs_col_sum bit for bit; only the grouping of the dot
+// products differs from the two-kernel loop.
+#pragma once
+#include "cg_kernel.cuh"
+
+namespace b200 {
+
+constexpr int kXpThreads = 512;
+constexpr int kXpWarps = kXpThreads / 32;
+// dynamic shared memory per CTA: S blocks, M^-1 blocks, and seven vectors (x r p b D_f a z) of the owned cameras
+inline size_t xs_pcg_smem_bytes(int max_blocks, int max_cams) {
+  return sizeof(double) * (81 * static_cast<size_t>(max_blocks) + (81 + 7 * 9) * static_cast<size_t>(max_cams));
+}
+
+struct XsPcgArgs {
+  XsView v;
+  CgParams prm;
+  int reset;                  // residual reset period (iterations)
+  const int2* cta;            // [grid + 1] {first block row, first block} of each CTA
+  const int* warp_step;       // [grid * kXpWarps + 1] first product step of each warp
+  int max_blocks, max_cams;   // the shared-memory geometry: the largest CTA's blocks and cameras
+  const double* minv;         // [C][81] M^-1
+  const double* rhs;          // [9C]
+  const double* Df;           // [9C] or null
+  double *x, *z;              // [9C]
+  double* p[2];               // [9C] each: p of the even / odd iterations
+  double* red;                // [grid][4] per-CTA partials: p.q | x.(b+r), r.r, r.z
+  CgState* st;
+#ifdef B200_DEV_KNOBS
+  long long* stamps;          // B200_XS_STAMPS: clock64() cycles of CTA 0 by phase, accumulated over the solve (kXpPhases)
+#endif
+};
+
+// phases of the stamps: prologue and CG_BEGIN, product, wait at barrier 1, vector phase (with a reset's product and
+// barriers), wait at barrier 2, tests and the new p
+constexpr int kXpPhases = 6;
+#ifdef B200_DEV_KNOBS
+#define XP_STAMP(k)                                                   \
+  if (a.stamps != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {   \
+    const long long t_now = clock64();                                \
+    a.stamps[k] += t_now - t_mark;                                    \
+    t_mark = t_now;                                                   \
+  }
+#else
+#define XP_STAMP(k)
+#endif
+
+__global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
+  cg::grid_group grid = cg::this_grid();
+#ifdef B200_DEV_KNOBS
+  long long t_mark = clock64();
+#endif
+  extern __shared__ double smem[];
+  __shared__ double scratch[kXpWarps][3];
+  __shared__ double s_tot[4];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int e = lane / 9, w = lane - 9 * (lane / 9);   // e == 3: lanes 27..31, no block
+  const int2 lo = a.cta[blockIdx.x], hi = a.cta[blockIdx.x + 1];
+  const int r0 = lo.x, ncam = hi.x - lo.x, nent = 9 * ncam, b0 = lo.y, nblk = hi.y - lo.y;
+  double* s_S = smem;
+  double* s_minv = s_S + 81 * static_cast<size_t>(a.max_blocks);
+  double* s_x = s_minv + 81 * static_cast<size_t>(a.max_cams);
+  double* s_r = s_x + 9 * a.max_cams;
+  double* s_p = s_r + 9 * a.max_cams;
+  double* s_b = s_p + 9 * a.max_cams;
+  double* s_d = s_b + 9 * a.max_cams;
+  double* s_a = s_d + 9 * a.max_cams;
+  double* s_z = s_a + 9 * a.max_cams;
+  const XsView& v = a.v;
+  const size_t o0 = 9 * static_cast<size_t>(r0);   // first owned entry
+  const bool writer = blockIdx.x == 0 && tid == 0;
+  const int k0 = __ldg(a.warp_step + blockIdx.x * kXpWarps + warp), k1 = __ldg(a.warp_step + blockIdx.x * kXpWarps + warp + 1);
+
+  // ---- prologue: the CTA's blocks of S (contiguous: block rows own their blocks) and M^-1 blocks, b and D_f
+  {
+    const double* src = v.S + 81 * static_cast<size_t>(b0);
+    const int n = 81 * nblk;
+    int i = tid;
+    for (; i + 3 * kXpThreads < n; i += 4 * kXpThreads) {
+      double t[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) t[k] = __ldcg(src + i + k * kXpThreads);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) s_S[i + k * kXpThreads] = t[k];
+    }
+    for (; i < n; i += kXpThreads) s_S[i] = __ldcg(src + i);
+    for (int k = tid; k < 81 * ncam; k += kXpThreads) s_minv[k] = __ldcg(a.minv + 81 * static_cast<size_t>(r0) + k);
+  }
+  for (int k = tid; k < nent; k += kXpThreads) {
+    s_b[k] = a.rhs[o0 + k];
+    s_d[k] = a.Df != nullptr ? a.Df[o0 + k] : 0.0;
+    s_p[k] = 0.0;
+  }
+  auto load_s = [&](int2 d, int e, int w, double* s) {
+    const bool in = xs_lane_in(d, e);
+    const double* sb = s_S + 81 * (in ? d.x + e - b0 : 0) + w;
+#pragma unroll
+    for (int u = 0; u < 9; ++u) s[u] = in ? sb[9 * u] : 0.0;
+  };
+  auto keep_row = [&](int i, int u, double av, double) { s_a[9 * (i - r0) + u] = av; };
+  // z = M^-1 r of the owned cameras (s_r complete), and the partials x.(b+r), r.r, r.z into red[CTA][1..3]
+  auto precondition = [&]() {
+    __syncthreads();
+    double accQ = 0.0, accR = 0.0, accRho = 0.0;
+    for (int k = tid; k < nent; k += kXpThreads) {
+      const int cl = k / 9, row = k - 9 * cl;
+      const double* m = s_minv + 81 * cl + 9 * row;
+      const double* rc = s_r + 9 * cl;
+      double zj = 0.0;
+#pragma unroll
+      for (int t = 0; t < 9; ++t) zj += m[t] * rc[t];
+      s_z[k] = zj;
+      a.z[o0 + k] = zj;
+      const double xj = s_x[k], rj = s_r[k];
+      accQ += xj * (s_b[k] + rj);
+      accR += rj * rj;
+      accRho += rj * zj;
+    }
+    cg_block_sum3<kXpWarps>(accQ, accR, accRho, scratch);
+    if (tid == 0) {
+      a.red[blockIdx.x * 4 + 1] = accQ;
+      a.red[blockIdx.x * 4 + 2] = accR;
+      a.red[blockIdx.x * 4 + 3] = accRho;
+    }
+  };
+
+  // ---- CG_BEGIN: x = 0, r = b, z = M^-1 r
+  for (int k = tid; k < nent; k += kXpThreads) {
+    s_x[k] = 0.0;
+    s_r[k] = s_b[k];
+    a.x[o0 + k] = 0.0;
+  }
+  precondition();
+  grid.sync();
+  double tot[3];
+  cg_totals(a.red, gridDim.x, 1, 3, tot, s_tot);
+  XP_STAMP(0);
+  double rho = 1.0, Q0 = 0.0, tol_r = 0.0, beta = 0.0;
+  int it = 0;
+  if (!cg_phase_c(a.prm, true, 0, rho, Q0, tol_r, tot[0], tot[1], tot[2], a.st, writer, &beta, &Q0, &tol_r)) return;
+  rho = tot[2];
+
+  for (;;) {
+    // ---- p of iteration it + 1 on the owned cameras; its share of D_f^2 p.p
+    double pq = 0.0;
+    for (int k = tid; k < nent; k += kXpThreads) {
+      const double pn = cg_next_p(it, s_z[k], beta, s_p[k]);
+      s_p[k] = pn;
+      a.p[(it + 1) & 1][o0 + k] = pn;
+      pq += s_d[k] * s_d[k] * pn * pn;
+    }
+    const double* p_prev = a.p[it & 1];   // p of iteration it, for the foreign columns
+    ++it;
+    __syncthreads();
+    // ---- product S p
+    {
+      XsWalk wk;
+      xs_walk_begin(v, k0, k1, e, w, load_s, wk);
+      pq += xs_walk(
+          v, k0, k1, lane, e, w, load_s,
+          [&](int j, int w) -> double {
+            const int l = j - r0;
+            if (l >= 0 && l < ncam) return s_p[9 * l + w];
+            const size_t o = 9 * static_cast<size_t>(j) + w;
+            return cg_next_p(it - 1, __ldcg(a.z + o), beta, __ldcg(p_prev + o));
+          },
+          keep_row, wk);
+    }
+    {
+      double d1 = 0.0, d2 = 0.0;
+      cg_block_sum3<kXpWarps>(pq, d1, d2, scratch);
+      if (tid == 0) a.red[blockIdx.x * 4] = pq;
+    }
+    XP_STAMP(1);
+    grid.sync();
+    XP_STAMP(2);
+    // ---- vector phase
+    double pq_tot, alpha = 0.0;
+    cg_totals(a.red, gridDim.x, 0, 1, &pq_tot, s_tot);
+    if (!cg_alpha(pq_tot, rho, it, a.st, writer, &alpha)) return;
+    const bool reset = it % a.reset == 0;
+    for (int k = tid; k < nent; k += kXpThreads) {
+      const double pj = s_p[k];
+      double xj = s_x[k];
+      xj += alpha * pj;
+      s_x[k] = xj;
+      a.x[o0 + k] = xj;
+      if (!reset) {
+        const double dj = s_d[k];
+        const double q = xs_col_sum(v.col_ptr, v.T, static_cast<int>(o0) + k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), pj)));
+        double rj = s_r[k];
+        rj -= alpha * q;
+        s_r[k] = rj;
+      }
+    }
+    if (reset) {
+      // r = b - S x: the product on x, whose every column is read back from its owner
+      grid.sync();
+      {
+        XsWalk wk;
+        xs_walk_begin(v, k0, k1, e, w, load_s, wk);
+        xs_walk(
+            v, k0, k1, lane, e, w, load_s, [&](int j, int w) { return __ldcg(a.x + 9 * static_cast<size_t>(j) + w); },
+            keep_row, wk);
+      }
+      grid.sync();
+      for (int k = tid; k < nent; k += kXpThreads) {
+        const double dj = s_d[k];
+        const double q = xs_col_sum(v.col_ptr, v.T, static_cast<int>(o0) + k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), s_x[k])));
+        s_r[k] = s_b[k] - q;
+      }
+    }
+    precondition();
+    XP_STAMP(3);
+    grid.sync();
+    XP_STAMP(4);
+    // ---- tests of iteration it, beta
+    cg_totals(a.red, gridDim.x, 1, 3, tot, s_tot);
+    if (!cg_phase_c(a.prm, false, it, rho, Q0, tol_r, tot[0], tot[1], tot[2], a.st, writer, &beta, &Q0, &tol_r)) return;
+    rho = tot[2];
+    XP_STAMP(5);
+  }
+}
+
+}  // namespace b200
