@@ -3,6 +3,7 @@ hot path for bundle adjustment: CUDA kernels + C ABI in csrc/ (libb200ba.so), ct
 host-side problem preparation in bal.py.  No CPU fallback: using the compute path without the built library
 or without a GPU raises."""
 from . import bal  # noqa: F401
-from .binding import (B200Error, Problem, lib, nccl_unique_id, plan_point_order, LIB_PATH, SYMBOLS,  # noqa: F401
-                      PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION, ITERATIVE_SCHUR, DENSE_SCHUR, LOSS_TRIVIAL, LOSS_HUBER,
+from .binding import (B200Error, Problem, lib, nccl_unique_id, plan_point_order, plan_sparse_schur, LIB_PATH, SYMBOLS,  # noqa: F401
+                      PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION, ITERATIVE_SCHUR, DENSE_SCHUR,
+                      SPARSE_SCHUR, SPARSE_STATS, LOSS_TRIVIAL, LOSS_HUBER,
                       LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR)

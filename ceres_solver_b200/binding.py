@@ -22,7 +22,10 @@ ERR_EVALUATION_FAILED = -3
 ERR_UNSUPPORTED = -6
 LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR = 0, 1, 2, 3
 PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION = 0, 1, 2, 3
-ITERATIVE_SCHUR, DENSE_SCHUR = 0, 1
+ITERATIVE_SCHUR, DENSE_SCHUR, SPARSE_SCHUR = 0, 1, 2
+# b200_plan_sparse_schur's statistics (B200_SPARSE_STAT_*), in order
+SPARSE_STATS = ("s_blocks", "l_blocks", "l_blocks_caller", "l_blocks_min_degree", "flops_caller", "flops_min_degree",
+                "supernodes", "tree_height", "order", "factor_bytes")
 LOSS_TRIVIAL, LOSS_HUBER = 0, 1
 
 
@@ -76,7 +79,7 @@ class KernelStat(C.Structure):
 
 # Every symbol include/b200ba.h declares (tests/test_abi.py checks the library exports all of them).
 SYMBOLS = [
-    "b200_plan_point_order", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
+    "b200_plan_point_order", "b200_plan_sparse_schur", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
     "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
@@ -129,6 +132,21 @@ def plan_point_order(num_cameras, num_points, cam_idx, pt_idx, num_chunks=132):
     choice = C.c_int()
     _check(lib().b200_plan_point_order(C.byref(d), int(num_chunks), perm.ctypes.data_as(_ip), metrics, C.byref(choice)))
     return perm, [int(m) for m in metrics], choice.value
+
+
+def plan_sparse_schur(num_cameras, num_points, cam_idx, pt_idx):
+    """Host-only: the symbolic analysis b200_sparse_schur_solve runs for this structure.  Returns (camera elimination order,
+    dict of SPARSE_STATS)."""
+    cam = np.ascontiguousarray(cam_idx, dtype=np.int32)
+    pt = np.ascontiguousarray(pt_idx, dtype=np.int32)
+    d = BaDesc()
+    d.num_cameras, d.num_points, d.num_observations = int(num_cameras), int(num_points), len(cam)
+    d.cam_idx = cam.ctypes.data_as(_ip)
+    d.pt_idx = pt.ctypes.data_as(_ip)
+    perm = np.zeros(int(num_cameras), dtype=np.int32)
+    stats = (C.c_int64 * len(SPARSE_STATS))()
+    _check(lib().b200_plan_sparse_schur(C.byref(d), perm.ctypes.data_as(_ip), stats))
+    return perm, {k: int(v) for k, v in zip(SPARSE_STATS, stats)}
 
 
 def nccl_unique_id():
@@ -258,6 +276,13 @@ class Problem:
         s = SolverSummary()
         bp = _d(_f64(b)) if b is not None else None
         _check(lib().b200_dense_schur_solve(self.h, bp, _d(_f64(D)), _d(x), C.byref(s)))
+        return x, s.num_iterations, s.termination_type
+
+    def sparse_schur_solve(self, b, D):
+        x = np.full(self.num_parameters, np.nan)
+        s = SolverSummary()
+        bp = _d(_f64(b)) if b is not None else None
+        _check(lib().b200_sparse_schur_solve(self.h, bp, _d(_f64(D)), _d(x), C.byref(s)))
         return x, s.num_iterations, s.termination_type
 
     def model_cost_change(self, step):

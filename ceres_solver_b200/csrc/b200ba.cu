@@ -40,6 +40,8 @@
 #include "dense_schur.cuh"
 #include "explicit_schur.cuh"
 #include "plan.cuh"
+#include "sparse_plan.cuh"
+#include "sparse_schur.cuh"
 
 using namespace b200;
 
@@ -255,6 +257,16 @@ struct b200_handle {
   bool xs_pcg = false;
   XsPcgArgs xpa{};             // the plan's geometry and the device arrays; the solve fills in its options and vectors
   size_t xs_pcg_smem = 0;
+  // SPARSE_SCHUR (sparse_plan.cuh, sparse_schur.cuh): the row structure in the internal order, kept for the symbolic analysis
+  // of the first sparse solve, and what that analysis uploads
+  std::vector<int> h_cam_idx, h_pt_idx, h_pt_ptr;
+  bool sp_ready = false;
+  bool xs_arrays = false;       // the arrays xs_assemble_dev reads exist (explicit plan, or uploaded by the sparse analysis)
+  SparseView spv{};
+  long long sp_storage = 0;     // doubles of factor storage
+  int sp_grid = 0;
+  size_t sp_smem = 0;
+  int* d_sp_cnt_init = nullptr;
   double* d_red = nullptr;    // per-CTA partial sums of cg_vector_kernel
   // multi-GPU exchange of the per-iteration partial products over NVLink peer memory (cg_kernel.cuh: xchg_push_kernel +
   // the gather in cg_vector_kernel); replaces the ncclAllReduce inside the PCG iteration when every peer could be mapped
@@ -1000,6 +1012,116 @@ int dense_schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, 
   return B200_OK;
 }
 
+// The symbolic analysis of SPARSE_SCHUR (sparse_plan.cuh), once per handle: the block pattern of S from the row structure
+// (the same xs_pattern b200_create ran), the plan, and its upload.  A handle whose plan kept S implicit gets the arrays
+// xs_assemble_dev reads here (not those of the explicit product).
+constexpr double kFactorMaxBytes = 48.0 * (1ull << 30);   // the dense path's cap
+static_assert(kSpMaxCols == 9 * kSnMaxCams && kSpThreads == 32 * 8 && kSpTileRows == 64,
+              "an update tile: two column blocks per warp, two rows per lane");
+int sparse_analyse(b200_handle* h) {
+  XsPattern xp;
+  xs_pattern(h->C, h->N, h->h_cam_idx.data(), h->h_pt_idx.data(), h->h_pt_ptr.data(), &xp);
+  SparsePlan sp;
+  plan_sparse_schur(h->C, xp.blk_row, xp.blk_col, &sp);
+  if (8.0 * static_cast<double>(sp.storage) > kFactorMaxBytes)
+    return fail(B200_ERR_UNSUPPORTED, "sparse factor of %d cameras needs %.1f GB", h->C, 8.0 * static_cast<double>(sp.storage) / 1e9);
+  if (!h->xs_arrays) {
+    XsView& x = h->xsv;
+    x.C = h->C;
+    x.num_blocks = static_cast<int>(xp.blk_row.size());
+    OK(upload(h, xp.blk_row, &x.blk_row));
+    OK(upload(h, xp.blk_col, &x.blk_col));
+    OK(upload(h, xp.pair_ptr, &x.pair_ptr));
+    OK(upload(h, xp.pairs, &x.pairs));
+    OK(dev_alloc(h, &x.S, 81 * static_cast<size_t>(x.num_blocks)));
+    std::vector<int> order;
+    h->num_xs_long = xs_assembly_order(xp, &order);
+    h->num_xs_short = x.num_blocks - h->num_xs_long;
+    OK(upload(h, order, &h->d_xs_order));
+    h->xs_arrays = true;
+  }
+  SparseView& v = h->spv;
+  v.C = h->C;
+  v.ns = sp.ns;
+  OK(upload(h, sp.pinv, &v.pinv));
+  OK(upload(h, sp.sn_first, &v.sn_first));
+  OK(upload(h, sp.row_ptr, &v.row_ptr));
+  OK(upload(h, sp.rows, &v.rows));
+  OK(upload(h, sp.val, &v.val));
+  OK(upload(h, sp.upd_ptr, &v.upd_ptr));
+  OK(upload(h, sp.upd, &v.upd));
+  OK(upload(h, sp.ntf_ptr, &v.ntf_ptr));
+  OK(upload(h, sp.ntf, &v.ntf));
+  OK(upload(h, sp.blk_off, &v.blk_off));
+  OK(upload(h, sp.blk_ld, &v.blk_ld));
+  OK(upload(h, sp.cnt, &h->d_sp_cnt_init));
+  OK(dev_alloc(h, &v.L, static_cast<size_t>(sp.storage)));
+  OK(dev_alloc(h, &v.v, 9 * static_cast<size_t>(h->C)));
+  OK(dev_alloc(h, &v.cnt, sp.cnt.size()));
+  OK(dev_alloc(h, &v.ticket, 2));
+  v.fail = v.ticket + 1;
+  h->sp_storage = sp.storage;
+  h->sp_smem = sparse_smem_bytes(sp.max_width);
+  int per_sm = 0;
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sparse_factor_kernel, kSpThreads, h->sp_smem));
+  if (per_sm < 1) return fail(B200_ERR_UNSUPPORTED, "no CTA of the sparse factorisation fits an SM (%zu bytes of shared memory)", h->sp_smem);
+  h->sp_grid = std::max(1, std::min(per_sm * h->sm_count, 2 * sp.ns));
+  CU(cudaStreamSynchronize(h->stream));   // the host vectors above go out of scope
+  if (getenv("B200_VERBOSE") != nullptr) {
+    const int64_t* st = sp.stats;
+    fprintf(stderr,
+            "[b200ba] sparse S plan: %lld blocks of S, L %lld blocks (caller's order %lld, minimum degree %lld), flops caller %.3g / "
+            "minimum degree %.3g -> %s, %d supernodes (widest %d columns), tree height %lld, factor %.1f MB, %d CTAs\n",
+            static_cast<long long>(st[B200_SPARSE_STAT_S_BLOCKS]), static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS]),
+            static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS_CALLER]), static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS_MIN_DEGREE]),
+            static_cast<double>(st[B200_SPARSE_STAT_FLOPS_CALLER]), static_cast<double>(st[B200_SPARSE_STAT_FLOPS_MIN_DEGREE]),
+            st[B200_SPARSE_STAT_ORDER] ? "minimum degree" : "caller's order", sp.ns, sp.max_width,
+            static_cast<long long>(st[B200_SPARSE_STAT_TREE_HEIGHT]), 8.0 * static_cast<double>(sp.storage) / 1e6, h->sp_grid);
+  }
+  h->sp_ready = true;
+  return B200_OK;
+}
+
+// SparseSchurComplementSolver (schur_complement_solver.cc:205-335) on device pointers: S by xs_assemble_kernel, scattered with
+// D_f^2 into the supernodal factor, factored and solved by sparse_factor_kernel, back substitution by the implicit-Schur kernels.
+int sparse_schur_solve_dev(b200_handle* h, const double* d_b, const double* d_D, double* d_x, b200_solver_summary* summary) {
+  if (h->world > 1) return fail(B200_ERR_UNSUPPORTED, "the explicit Schur complement is single-GPU");
+  if (!h->sp_ready) OK(sparse_analyse(h));
+  OK(schur_init_dev(h, d_b, d_D));   // (E'E + D^2)^-1 and the reduced right-hand side
+  if (!h->xs_ready) OK(xs_assemble_dev(h));
+  const double* Df = d_D != nullptr ? d_D + 3 * static_cast<size_t>(h->P) : nullptr;
+  SparseView& v = h->spv;
+  CU(cudaMemsetAsync(v.L, 0, sizeof(double) * static_cast<size_t>(h->sp_storage), h->stream));
+  CU(cudaMemcpyAsync(v.cnt, h->d_sp_cnt_init, sizeof(int) * 2 * static_cast<size_t>(v.ns), cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemsetAsync(v.ticket, 0, 2 * sizeof(int), h->stream));
+  OK(launch(h, K_SPARSE_SCATTER, [&] {
+    const int g = std::max(1, std::min((h->xsv.num_blocks + 7) / 8, h->sm_count * 8));
+    sparse_scatter_kernel<<<g, 256, 0, h->stream>>>(v, h->xsv, Df, h->d_rhs);
+  }));
+  cudaError_t le = cudaSuccess;
+  OK(launch(h, K_SPARSE_FACTOR, [&] {
+    void* args[] = {&v};
+    le = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(sparse_factor_kernel), dim3(h->sp_grid), dim3(kSpThreads), args,
+                                     h->sp_smem, h->stream);
+  }));
+  CU(le);
+  CU(cudaMemcpyAsync(h->h_fail, v.fail, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  summary->num_iterations = 1;   // schur_complement_solver.cc:154
+  summary->residual_norm = 0.0;
+  if (h->h_fail[0] != 0) {   // not positive definite: CHOLMOD_NOT_POSDEF, suitesparse.cc:311-313 -> FAILURE
+    summary->termination_type = B200_LS_FAILURE;
+    return B200_OK;
+  }
+  summary->termination_type = B200_LS_SUCCESS;
+  OK(launch(h, K_SPARSE_SCATTER, [&] {
+    sparse_gather_kernel<<<(9 * h->C + 255) / 256, 256, 0, h->stream>>>(v, h->d_sol);
+  }, false));
+  OK(back_substitute_dev(h, d_b, h->d_sol, d_x));
+  CU(cudaMemcpyAsync(d_x + 3 * static_cast<size_t>(h->P), h->d_sol, sizeof(double) * 9 * h->C, cudaMemcpyDeviceToDevice, h->stream));
+  return B200_OK;
+}
+
 int reduce_partials(b200_handle* h, int blocks, int slots, unsigned op_mask, double* host_out, bool across_ranks) {
   OK(launch(h, K_LM_VEC, [&] { reduce_final_kernel<<<1, 32, 0, h->stream>>>(blocks, slots, op_mask, h->d_partial, h->d_scalars + 8); }));
 #ifdef B200_WITH_NCCL
@@ -1254,6 +1376,7 @@ int set_func_attributes(int smem_optin) {
   OK(raise_smem_limit(diag_blocks_v2_kernel<true>, lim));
   OK(raise_smem_limit(diag_blocks_v2_kernel<false>, lim));
   OK(raise_smem_limit(xs_pcg_kernel, lim));
+  OK(raise_smem_limit(sparse_factor_kernel, lim));
   return B200_OK;
 }
 
@@ -1295,6 +1418,24 @@ int b200_plan_point_order(const b200_ba_desc* desc, int num_chunks, int32_t* per
   if (metrics_out != nullptr)
     for (int k = 0; k < 4; ++k) metrics_out[k] = m[k];
   if (choice_out != nullptr) *choice_out = choice;
+  return B200_OK;
+}
+
+int b200_plan_sparse_schur(const b200_ba_desc* desc, int32_t* cam_perm_out, int64_t stats_out[B200_SPARSE_STATS]) {
+  if (desc == nullptr || desc->cam_idx == nullptr || desc->pt_idx == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  const int C = desc->num_cameras, P = desc->num_points;
+  const int N = static_cast<int>(desc->num_observations);
+  if (C <= 0 || P <= 0 || N <= 0) return fail(B200_ERR_INVALID_ARGUMENT, "empty problem");
+  std::vector<int> ptr;
+  OK(validate_rows(desc, &ptr));
+  XsPattern xp;   // the block pattern of S does not depend on the point order: the caller's rows give the handle's pattern
+  xs_pattern(C, N, desc->cam_idx, desc->pt_idx, ptr.data(), &xp);
+  SparsePlan sp;
+  plan_sparse_schur(C, xp.blk_row, xp.blk_col, &sp);
+  if (cam_perm_out != nullptr)
+    for (int k = 0; k < C; ++k) cam_perm_out[k] = sp.perm[k];
+  if (stats_out != nullptr)
+    for (int k = 0; k < B200_SPARSE_STATS; ++k) stats_out[k] = sp.stats[k];
   return B200_OK;
 }
 
@@ -1540,6 +1681,12 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     }
   }
   CU(cudaStreamSynchronize(h->stream));
+  h->xs_arrays = h->xs;
+  if (world == 1) {   // the uploads above are complete: the plan's host copies can move
+    h->h_cam_idx = std::move(pl.cam_idx);
+    h->h_pt_idx = std::move(pl.pt_idx);
+    h->h_pt_ptr = std::move(pl.pt_ptr);
+  }
 
   for (int k = 0; k < K_COUNT; ++k) h->grid_tile[k] = std::max(1, std::min(h->num_tiles, h->sm_count * 4));
   h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<true>, tile_smem_bytes<3, 1>());
@@ -1920,6 +2067,22 @@ int b200_dense_schur_solve(b200_handle* h, const double* b, const double* D, dou
   return B200_OK;
 }
 
+int b200_sparse_schur_solve(b200_handle* h, const double* b, const double* D, double* x, b200_solver_summary* summary) {
+  if (h == nullptr || x == nullptr || summary == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  if (b == nullptr && !h->residuals_resident)
+    return fail(B200_ERR_INVALID_ARGUMENT, "b == NULL means the residuals of the last b200_evaluate, and there are none");
+  CU(cudaSetDevice(h->device));
+  const double* d_b = h->d_residuals;
+  if (b != nullptr) {
+    OK(up_rows(h, h->d_b, b));
+    d_b = h->d_b;
+  }
+  if (D != nullptr) OK(up_params(h, h->d_D, D));
+  OK(sparse_schur_solve_dev(h, d_b, D != nullptr ? h->d_D : nullptr, h->d_y, summary));
+  if (summary->termination_type == B200_LS_SUCCESS) OK(down_params(h, x, h->d_y));
+  return B200_OK;
+}
+
 int b200_schur_init(b200_handle* h, const double* b, const double* D) {
   if (h == nullptr || b == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   CU(cudaSetDevice(h->device));
@@ -2134,6 +2297,7 @@ int b200_lm_solve(b200_handle* h, const b200_lm_options* opt, double* state_inou
       // (levenberg_marquardt_strategy.cc:108 pre-fills the step with NaN so that a solver that silently writes nothing is
       //  caught; here the solve either fills sol or reports FAILURE / FATAL_ERROR, which the code below checks)
       if (opt->linear_solver_type == B200_DENSE_SCHUR) OK(b200_dense_schur_solve(h, nullptr, lmD.data(), sol.data(), &ls));
+      else if (opt->linear_solver_type == B200_SPARSE_SCHUR) OK(b200_sparse_schur_solve(h, nullptr, lmD.data(), sol.data(), &ls));
       else OK(b200_schur_solve(h, nullptr /* residuals of the last evaluate, still in HBM */, lmD.data(), &so, sol.data(), &ls));
       if (ls.termination_type != B200_LS_FAILURE && ls.termination_type != B200_LS_FATAL_ERROR) {
         // step = -sol, delta = step * scaling, candidate = x + delta (Evaluator::Plus on Euclidean blocks) and the two
@@ -2179,6 +2343,7 @@ int b200_lm_solve(b200_handle* h, const b200_lm_options* opt, double* state_inou
                                                                           opt->min_lm_diagonal, opt->max_lm_diagonal, radius);
       }));
       if (opt->linear_solver_type == B200_DENSE_SCHUR) OK(dense_schur_solve_dev(h, h->d_residuals, h->d_lmD, h->d_y, &ls));
+      else if (opt->linear_solver_type == B200_SPARSE_SCHUR) OK(sparse_schur_solve_dev(h, h->d_residuals, h->d_lmD, h->d_y, &ls));
       else OK(schur_solve_dev(h, h->d_residuals, h->d_lmD, &so, h->d_y, &ls));
     }
     reuse_diagonal = true;

@@ -55,13 +55,16 @@ enum KernelId {
   K_PMV_LEFT_E,
   K_PMV_LEFT_F,
   K_SCHUR_PCG,
+  K_SPARSE_SCATTER,
+  K_SPARSE_FACTOR,
   K_MISC,
   K_COUNT
 };
 const char* const kKernelNames[K_COUNT] = {"evaluate_jacobian", "evaluate_cost", "squared_column_norm", "scale_columns",
                                            "jacobian_multiply", "jacobian_t_multiply", "jtj_multiply", "schur_init",
                                            "schur_multiply", "schur_multiply_big_points", "camera_reduce", "schur_diag_blocks", "invert_9x9", "back_substitute",
-                                           "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg", "misc"};
+                                           "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg",
+                                           "sparse_scatter", "sparse_factor", "misc"};
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.
@@ -257,6 +260,20 @@ inline void xs_pattern(int C, int N, const int* cam_idx, const int* pt_idx, cons
   xp->cols.resize(static_cast<size_t>(nb));
   for (int b = 0; b < nb; ++b)
     xp->cols[b] = make_int2(xp->blk_col[b], xp->blk_col[b] != xp->blk_row[b] ? fill[xp->blk_col[b]]++ : -1);
+}
+
+// The order xs_assemble_dev assembles the blocks in: the blocks with long pair lists (the diagonal ones, mostly) first, one
+// CTA each; then one warp per block.  Returns the number of long blocks.
+inline int xs_assembly_order(const XsPattern& xp, std::vector<int>* order) {
+  const int nb = static_cast<int>(xp.blk_row.size());
+  order->clear();
+  order->reserve(static_cast<size_t>(nb));
+  for (int b = 0; b < nb; ++b)
+    if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] > kXsLongPairs) order->push_back(b);
+  const int num_long = static_cast<int>(order->size());
+  for (int b = 0; b < nb; ++b)
+    if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] <= kXsLongPairs) order->push_back(b);
+  return num_long;
 }
 
 // ---- Internal point order.  The fast kernels give every persistent CTA a contiguous run of points and keep the cameras
@@ -855,13 +872,7 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
       else if (knobs.xs_resident == 0) pl.xs_pcg_why = "B200_XS_RESIDENT=0";
       else pl.xs_pcg = true;
     }
-    // the blocks with long pair lists (the diagonal ones, mostly) first, one CTA each; then one warp per block
-    pl.xs_order.reserve(static_cast<size_t>(nb));
-    for (int b = 0; b < nb; ++b)
-      if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] > kXsLongPairs) pl.xs_order.push_back(b);
-    pl.num_xs_long = static_cast<int>(pl.xs_order.size());
-    for (int b = 0; b < nb; ++b)
-      if (xp.pair_ptr[b + 1] - xp.pair_ptr[b] <= kXsLongPairs) pl.xs_order.push_back(b);
+    pl.num_xs_long = xs_assembly_order(xp, &pl.xs_order);
   }
 
   // Algorithmic (compulsory) bytes per launch, SURVEY §8d with this layout: J values 192 B/row + 4 B camera

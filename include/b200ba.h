@@ -49,9 +49,9 @@ enum {
   B200_PRECOND_SCHUR_POWER_SERIES_EXPANSION = 3 /* power_series_expansion_preconditioner.cc:57-82 */
 };
 enum { B200_LOSS_TRIVIAL = 0, B200_LOSS_HUBER = 1 };
-/* LinearSolverType subset (include/ceres/types.h): the implicit iterative solver and the exact solve on the explicit
- * reduced camera system (DENSE_SCHUR; stands in for SPARSE_SCHUR too: both are exact solves of the same system). */
-enum { B200_ITERATIVE_SCHUR = 0, B200_DENSE_SCHUR = 1 };
+/* LinearSolverType subset (include/ceres/types.h): the implicit iterative solver and the two exact solves of the explicit
+ * reduced camera system, by a dense Cholesky (DENSE_SCHUR) and by a block-sparse supernodal Cholesky (SPARSE_SCHUR). */
+enum { B200_ITERATIVE_SCHUR = 0, B200_DENSE_SCHUR = 1, B200_SPARSE_SCHUR = 2 };
 
 /* Problem structure = what the adapters read off the reduced ceres::internal::Program
  * (residual_block->parameter_blocks()[j]->index(), SnavelyReprojectionError::observed_x/y,
@@ -82,6 +82,26 @@ typedef struct b200_ba_desc {
  * metrics_out = distinct cameras per 1/num_chunks of the rows, summed, for {caller's order, by camera arc, by mean camera,
  * by smallest camera}; *choice_out = which of the four was taken (0 = the caller's order is kept). */
 int b200_plan_point_order(const b200_ba_desc* desc, int num_chunks, int32_t* perm_out, int64_t metrics_out[4], int* choice_out);
+/* The symbolic analysis b200_sparse_schur_solve runs at its first call on a handle of this structure.  Host-only, needs no GPU:
+ * cam_perm_out[k] = camera eliminated k-th ([C], may be NULL); stats_out (may be NULL), indexed by B200_SPARSE_STAT_*:
+ * blocks of the upper triangle of S (diagonal included); blocks of L (diagonal included) in the chosen order, in the caller's
+ * order and in the minimum-degree order; factor flops in the caller's and in the minimum-degree order; supernodes; height of
+ * the elimination tree (nodes on its longest path); which order was taken (0 the caller's, 1 minimum degree: the one of
+ * fewer flops, the caller's on a tie; minimum degree is tried up to 32768 cameras); bytes of factor storage. */
+enum {
+  B200_SPARSE_STAT_S_BLOCKS = 0,
+  B200_SPARSE_STAT_L_BLOCKS,
+  B200_SPARSE_STAT_L_BLOCKS_CALLER,
+  B200_SPARSE_STAT_L_BLOCKS_MIN_DEGREE,
+  B200_SPARSE_STAT_FLOPS_CALLER,
+  B200_SPARSE_STAT_FLOPS_MIN_DEGREE,
+  B200_SPARSE_STAT_SUPERNODES,
+  B200_SPARSE_STAT_TREE_HEIGHT,
+  B200_SPARSE_STAT_ORDER,
+  B200_SPARSE_STAT_FACTOR_BYTES,
+  B200_SPARSE_STATS
+};
+int b200_plan_sparse_schur(const b200_ba_desc* desc, int32_t* cam_perm_out, int64_t stats_out[B200_SPARSE_STATS]);
 int b200_nccl_unique_id(void* out128);
 int b200_create(const b200_ba_desc* desc, b200_handle** out);
 void b200_destroy(b200_handle* h);
@@ -162,6 +182,13 @@ int b200_schur_solve(b200_handle* h, const double* b, const double* D, const b20
  * Single GPU, 9C up to ~75k.  summary: num_iterations 1, SUCCESS or FAILURE (S not positive definite). b == NULL as above. */
 int b200_dense_schur_solve(b200_handle* h, const double* b, const double* D, double* x, b200_solver_summary* summary);
 
+/* SparseSchurComplementSolver::SolveImpl (schur_complement_solver.cc:205-335): the same explicit S, assembled block-sparse on
+ * the device, factored by a supernodal Cholesky in a fill-reducing camera order (b200_plan_sparse_schur; analysed once per
+ * handle, at the first call), two triangular solves and the back substitution.  Same contract as b200_dense_schur_solve:
+ * num_iterations 1, residual_norm 0, FAILURE without writing x when S + D_f^2 is not positive definite (CHOLMOD_NOT_POSDEF,
+ * suitesparse.cc:311-313); single GPU, factor storage up to 48 GB (B200_ERR_UNSUPPORTED otherwise); b == NULL as above. */
+int b200_sparse_schur_solve(b200_handle* h, const double* b, const double* D, double* x, b200_solver_summary* summary);
+
 /* Finer-grained pieces of the same solve, for parity tests (each mirrors one reference class):
  *   ImplicitSchurComplement::Init / rhs / RightMultiplyAndAccumulate / BackSubstitute
  *     (implicit_schur_complement.cc:49-97, :251-276, :106-144, :208-243)
@@ -181,7 +208,7 @@ typedef struct b200_lm_options { /* Solver::Options subset, include/ceres/solver
   int32_t max_num_iterations;              /* bundle_adjuster.cc:121 (5) */
   int32_t jacobi_scaling;                  /* 1 */
   int32_t max_num_consecutive_invalid_steps; /* 5 */
-  int32_t linear_solver_type;        /* B200_ITERATIVE_SCHUR (default) or B200_DENSE_SCHUR */
+  int32_t linear_solver_type;        /* B200_ITERATIVE_SCHUR (default), B200_DENSE_SCHUR or B200_SPARSE_SCHUR */
   double eta;                              /* 1e-2 */
   double initial_trust_region_radius;      /* 1e4 */
   double max_trust_region_radius;          /* 1e16 */

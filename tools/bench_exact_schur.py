@@ -1,0 +1,105 @@
+"""The two exact LM-step solvers, DENSE_SCHUR (b200_dense_schur_solve: dense S, cuSOLVER Cholesky) and SPARSE_SCHUR
+(b200_sparse_schur_solve: block-sparse S, supernodal Cholesky), on the same handle of each problem: time per solve from a host
+clock around synchronised calls and from the CUDA-event stats of a profiled pass, LM iterations per second of b200_lm_solve
+with each solver type, the symbolic statistics and the host analysis time, and the card's name and power limit.
+
+    python tools/bench_exact_schur.py [--reps 5] [--lm-iterations 5] [--problems ladybug-1723,...] [--out results.json]
+
+One JSON line per problem on stdout.  Needs an H100; nothing is written unless --out is given.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import ceres_solver_b200 as cs  # noqa: E402
+from ceres_solver_b200 import bal as B  # noqa: E402
+
+PROBLEMS = ["ladybug-1723", "venice-1778", "trafalgar-257", "ladybug-1723-random", "c16"]
+
+
+def card():
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return out.stdout.strip().splitlines()[0] if out.returncode == 0 and out.stdout.strip() else "unknown"
+
+
+def load(name):
+    if name == "c16":
+        return B.normalize(B.read_bal(os.path.join(ROOT, "tests", "golden", "problem-16-22106-pre.txt.bz2")))
+    return B.synthetic(name)
+
+
+def timed_solves(gpu, solve, b, D, reps):
+    solve(b, D)   # warm-up (the sparse analysis runs at the first call)
+    gpu.synchronize()
+    t = time.perf_counter()
+    for _ in range(reps):
+        x, _, term = solve(b, D)
+    ms = 1e3 * (time.perf_counter() - t) / reps
+    gpu.stats_reset()
+    gpu.profile(True)
+    for _ in range(reps):
+        solve(b, D)
+    gpu.synchronize()
+    gpu.profile(False)
+    kernels = {k: round(v["ms"] / reps, 3) for k, v in gpu.stats().items() if v["launches"] > 0}
+    return x, term, ms, kernels
+
+
+def lm_rate(gpu, state, solver_type, iterations):
+    o = gpu.lm_options(max_num_iterations=iterations)
+    o.linear_solver_type = solver_type
+    gpu.lm_solve(state, gpu.lm_options(max_num_iterations=1, linear_solver_type=solver_type))   # warm-up
+    gpu.synchronize()
+    t = time.perf_counter()
+    _, recs = gpu.lm_solve(state, o)
+    dt = time.perf_counter() - t
+    return (len(recs) - 1) / dt, recs[-1]["cost"]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--lm-iterations", type=int, default=5)
+    ap.add_argument("--problems", default=",".join(PROBLEMS))
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    device = card()
+    results = []
+    for name in a.problems.split(","):
+        bal = load(name)
+        rp = B.ReducedProgram(bal)
+        state = rp.state(bal)
+        t = time.perf_counter()
+        _, st = cs.plan_sparse_schur(rp.C, rp.P, rp.row_cam, rp.row_pt)
+        analysis_ms = 1e3 * (time.perf_counter() - t)
+        gpu = cs.Problem(rp.C, rp.P, rp.row_cam, rp.row_pt, rp.row_obs)
+        ok, _, res, _ = gpu.evaluate(state)
+        assert ok
+        s = 1.0 / (1.0 + np.sqrt(gpu.squared_column_norm()))
+        gpu.scale_columns(s)
+        D = np.sqrt(np.clip(gpu.squared_column_norm(), 1e-6, 1e32) / 1e4)
+        row = dict(problem=name, device=device, C=rp.C, P=rp.P, N=rp.N, analysis_ms=round(analysis_ms, 2), **st)
+        xs, ts, row["sparse_ms"], row["sparse_kernels_ms"] = timed_solves(gpu, gpu.sparse_schur_solve, res, D, a.reps)
+        xd, td, row["dense_ms"], row["dense_kernels_ms"] = timed_solves(gpu, gpu.dense_schur_solve, res, D, a.reps)
+        row["terminations"] = [int(ts), int(td)]
+        row["relerr_sparse_dense"] = float(np.linalg.norm(xs - xd) / np.linalg.norm(xd))
+        row["lm_its_per_s_sparse"], row["lm_cost_sparse"] = lm_rate(gpu, state, cs.SPARSE_SCHUR, a.lm_iterations)
+        row["lm_its_per_s_dense"], row["lm_cost_dense"] = lm_rate(gpu, state, cs.DENSE_SCHUR, a.lm_iterations)
+        gpu.close()
+        print(json.dumps(row), flush=True)
+        results.append(row)
+    if a.out:
+        with open(a.out, "w") as f:
+            json.dump(results, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
