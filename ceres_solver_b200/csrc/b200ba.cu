@@ -1666,8 +1666,14 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
       a.v = x;
       OK(upload(h, pl.xs_pcg_cta, &a.cta));
       OK(upload(h, pl.xs_pcg_warp_step, &a.warp_step));
+      OK(upload(h, pl.xs_pcg_fptr, &a.fptr));
+      OK(upload(h, pl.xs_pcg_fcol, &a.fcol));
+      OK(upload(h, pl.xs_pcg_cols, &a.v.cols));   // the kernel's blocks address their columns CTA-locally
       a.max_blocks = pl.xs_pcg_max_blocks;
       a.max_cams = pl.xs_pcg_max_cams;
+      a.max_foreign = pl.xs_pcg_max_foreign;
+      a.max_steps = pl.xs_pcg_max_cta_steps;
+      a.stage_slots = pl.xs_pcg_stage_slots;
       OK(dev_alloc(h, &a.p[1], nc));   // the second p buffer; the first is d_p
       OK(dev_alloc(h, &a.red, static_cast<size_t>(prop.multiProcessorCount) * 4));
       h->xs_pcg_smem = pl.xs_pcg_smem;

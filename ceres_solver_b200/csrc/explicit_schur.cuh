@@ -171,12 +171,15 @@ struct XsStepData {
   int2 c;        // {j, T slot} of the lane's block ({0, -1}: no block)
   double s[9];   // S[u][w] of the lane's block, u = 0..8
 };
+// kShared: v.steps and v.cols point into shared memory (the resident PCG's staged copies), not at the global arrays
+template <bool kShared>
 __device__ __forceinline__ int2 xs_step_desc(const XsView& v, int k, int k1) {
-  return k < k1 ? __ldg(v.steps + k) : make_int2(0, 0);   // past the end: a step of no blocks
+  return k < k1 ? (kShared ? v.steps[k] : __ldg(v.steps + k)) : make_int2(0, 0);   // past the end: a step of no blocks
 }
 __device__ __forceinline__ bool xs_lane_in(int2 d, int e) { return e < ((d.y >> kXsStepCountShift) & 3); }
+template <bool kShared>
 __device__ __forceinline__ int2 xs_step_col(const XsView& v, int2 d, int e) {
-  return xs_lane_in(d, e) ? __ldg(v.cols + d.x + e) : make_int2(0, -1);
+  return xs_lane_in(d, e) ? (kShared ? v.cols[d.x + e] : __ldg(v.cols + d.x + e)) : make_int2(0, -1);
 }
 __device__ __forceinline__ void xs_step_s(const XsView& v, int2 d, int e, int w, double* s) {
   const bool in = xs_lane_in(d, e);
@@ -192,19 +195,20 @@ __device__ __forceinline__ void xs_step_s(const XsView& v, int2 d, int e, int w,
 // fills the lane's column of step d's block e, load_x(j, w) returns entry w of x_j, row_out(i, lane, a_i[lane], x_i[lane])
 // takes the row part of row i in lanes 0..8.  xs_walk_begin loads what does not depend on x (before a grid dependency
 // resolves); xs_walk returns the lane's share of x . S x (x_i . a_i over its rows, x_j . t_ij over its blocks).
+// kShared: the descriptors and column entries come from shared memory (xs_step_desc).
 struct XsWalk {
   XsStepData nx;   // step k + 1
   int2 d2, c2;     // step k + 2: descriptor and column entry
 };
-template <class LoadS>
+template <bool kShared = false, class LoadS>
 __device__ __forceinline__ void xs_walk_begin(const XsView& v, int k0, int k1, int e, int w, LoadS load_s, XsWalk& wk) {
-  wk.nx.d = xs_step_desc(v, k0, k1);
-  wk.nx.c = xs_step_col(v, wk.nx.d, e);
+  wk.nx.d = xs_step_desc<kShared>(v, k0, k1);
+  wk.nx.c = xs_step_col<kShared>(v, wk.nx.d, e);
   load_s(wk.nx.d, e, w, wk.nx.s);
-  wk.d2 = xs_step_desc(v, k0 + 1, k1);
-  wk.c2 = xs_step_col(v, wk.d2, e);
+  wk.d2 = xs_step_desc<kShared>(v, k0 + 1, k1);
+  wk.c2 = xs_step_col<kShared>(v, wk.d2, e);
 }
-template <class LoadS, class LoadX, class RowOut>
+template <bool kShared = false, class LoadS, class LoadX, class RowOut>
 __device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int lane, int e, int w, LoadS load_s, LoadX load_x,
                                           RowOut row_out, XsWalk& wk) {
   XsStepData& nx = wk.nx;
@@ -225,8 +229,8 @@ __device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int l
     nx.c = c2;
     load_s(nx.d, e, w, nx.s);
     nx_x = xs_lane_in(nx.d, e) ? load_x(nx.c.x, w) : 0.0;
-    d2 = xs_step_desc(v, k + 2, k1);
-    c2 = xs_step_col(v, d2, e);
+    d2 = xs_step_desc<kShared>(v, k + 2, k1);
+    c2 = xs_step_col<kShared>(v, d2, e);
     // a row begins with its diagonal block in lanes 0..8: their x_j is x_i
     if (d.y & kXsStepFirst)
 #pragma unroll
@@ -305,20 +309,28 @@ __global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v
   }
 }
 
-// q + the column part of entry k = 9j + w of S x: sum over the blocks (i, j), i < j, of t_ij[w] in order of i (their T
-// slots are contiguous), loaded 8 at a time.
-__device__ __forceinline__ double xs_col_sum(const int* __restrict__ col_ptr, const double* T, int k, double q) {
-  const int j = k / 9, w = k - 9 * (k / 9);
-  const int c0 = __ldg(col_ptr + j), c1 = __ldg(col_ptr + j + 1);
+// q + entry w of the column part over T slots [c0, c1): sum of t_ij[w] in slot order, i.e. in order of i (a column's
+// slots are contiguous), loaded 8 at a time.  src holds slot c at 9 (c - base): T itself (base 0, read with ld.global.cg,
+// as the product that wrote it may run in the same launch), or, kStaged, a copy of slots from `base` on in shared memory.
+template <bool kStaged>
+__device__ __forceinline__ double xs_col_sum(const double* src, int base, int c0, int c1, int w, double q) {
   for (int c = c0; c < c1; c += 8) {
     double t[8];
 #pragma unroll
-    for (int m = 0; m < 8; ++m) t[m] = c + m < c1 ? __ldcg(T + 9 * static_cast<size_t>(c + m) + w) : 0.0;
+    for (int m = 0; m < 8; ++m) {
+      const double* s = src + 9 * static_cast<size_t>(c + m - base) + w;
+      t[m] = c + m < c1 ? (kStaged ? *s : __ldcg(s)) : 0.0;
+    }
 #pragma unroll
     for (int m = 0; m < 8; ++m)
       if (c + m < c1) q += t[m];
   }
   return q;
+}
+// q + the column part of entry k = 9j + w of S x: sum over the blocks (i, j), i < j, of t_ij[w] in order of i.
+__device__ __forceinline__ double xs_col_sum(const int* __restrict__ col_ptr, const double* T, int k, double q) {
+  const int j = k / 9, w = k - 9 * (k / 9);
+  return xs_col_sum<false>(T, 0, __ldg(col_ptr + j), __ldg(col_ptr + j + 1), w, q);
 }
 
 // Completes a product outside the PCG: y += the column part held in T.

@@ -197,7 +197,14 @@ struct KernelPlan {
   bool xs_pcg = false;
   std::vector<int2> xs_pcg_cta;        // [sm_count + 1] {first block row, first block}
   std::vector<int> xs_pcg_warp_step;   // [sm_count * kXpWarps + 1] first step of each warp (into xs_steps)
-  int xs_pcg_max_blocks = 0, xs_pcg_max_cams = 0, xs_pcg_max_steps = 0;
+  std::vector<int> xs_pcg_fptr;        // [sm_count + 1] each CTA's foreign columns in xs_pcg_fcol
+  std::vector<int> xs_pcg_fcol;        // per CTA, ascending: the columns past its last row that its blocks touch
+  std::vector<int2> xs_pcg_cols;       // [blocks] {CTA-local column, T slot}: l < owned cameras n: camera first row + l,
+                                       // else foreign column l - n of the block's CTA
+  int xs_pcg_max_blocks = 0, xs_pcg_max_cams = 0, xs_pcg_max_steps = 0, xs_pcg_max_foreign = 0;
+  int xs_pcg_max_cta_steps = 0;        // the most product steps of a CTA
+  int xs_pcg_max_slots = 0;            // the most T slots of a CTA's owned columns
+  int xs_pcg_stage_slots = 0;          // ... that fit the shared memory left: a CTA with at most these stages them
   size_t xs_pcg_smem = 0;
   const char* xs_pcg_why = "";         // why the PCG is not resident
   double bytes_per_op[K_COUNT] = {};
@@ -813,8 +820,11 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
     // Resident PCG (xs_pcg.cuh): the block rows in G contiguous ranges with the smallest possible largest range in blocks
     // (the share of S a CTA holds in shared memory): the least capacity K at which filling the CTAs in row order, each up
     // to K blocks, needs at most G of them.  Within a CTA its rows go to the warps balanced by steps plus one per row, as
-    // above.  Resident when the largest CTA's blocks, M^-1 blocks and vectors fit one CTA's shared memory next to the
-    // static scratch, and one CTA of the kernel fits each SM.
+    // above.  Every CTA also gets the sorted list of its foreign columns (j past its last row: its blocks are in the upper
+    // triangle, so j below that is an owned camera) and every block its column as an index into [owned cameras | foreign
+    // columns].  Resident when the largest CTA's blocks (with their column entries), M^-1 blocks and vectors, the most
+    // foreign columns and the most product steps of a CTA fit one CTA's shared memory next to the static scratch, and
+    // one CTA of the kernel fits each SM.
     {
       const int G = lim.sm_count;
       std::vector<int> first_step(static_cast<size_t>(C) + 1, 0);
@@ -848,10 +858,28 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
         cur += row_blocks(i);
       }
       pl.xs_pcg_warp_step.assign(static_cast<size_t>(G) * kXpWarps + 1, first_step[C]);
+      pl.xs_pcg_fptr.assign(static_cast<size_t>(G) + 1, 0);
+      pl.xs_pcg_cols.resize(static_cast<size_t>(nb));
       for (int b = 0; b < G; ++b) {
         const int i0 = pl.xs_pcg_cta[b].x, i1 = pl.xs_pcg_cta[b + 1].x;
-        pl.xs_pcg_max_blocks = std::max(pl.xs_pcg_max_blocks, pl.xs_pcg_cta[b + 1].y - pl.xs_pcg_cta[b].y);
+        const int b0 = pl.xs_pcg_cta[b].y, b1 = pl.xs_pcg_cta[b + 1].y;
+        pl.xs_pcg_max_blocks = std::max(pl.xs_pcg_max_blocks, b1 - b0);
         pl.xs_pcg_max_cams = std::max(pl.xs_pcg_max_cams, i1 - i0);
+        pl.xs_pcg_max_cta_steps = std::max(pl.xs_pcg_max_cta_steps, first_step[i1] - first_step[i0]);
+        pl.xs_pcg_max_slots = std::max(pl.xs_pcg_max_slots, xp.col_ptr[i1] - xp.col_ptr[i0]);
+        std::vector<int> fc;
+        for (int k = b0; k < b1; ++k)
+          if (xp.blk_col[k] >= i1) fc.push_back(xp.blk_col[k]);
+        std::sort(fc.begin(), fc.end());
+        fc.erase(std::unique(fc.begin(), fc.end()), fc.end());
+        for (int k = b0; k < b1; ++k) {
+          const int j = xp.blk_col[k];
+          const int l = j < i1 ? j - i0 : (i1 - i0) + static_cast<int>(std::lower_bound(fc.begin(), fc.end(), j) - fc.begin());
+          pl.xs_pcg_cols[k] = make_int2(l, xp.cols[k].y);
+        }
+        pl.xs_pcg_fcol.insert(pl.xs_pcg_fcol.end(), fc.begin(), fc.end());
+        pl.xs_pcg_fptr[b + 1] = static_cast<int>(pl.xs_pcg_fcol.size());
+        pl.xs_pcg_max_foreign = std::max(pl.xs_pcg_max_foreign, static_cast<int>(fc.size()));
         double tot = 0.0, cum = 0.0;
         for (int i = i0; i < i1; ++i) tot += row_steps(i) + 1;
         int* ws = pl.xs_pcg_warp_step.data() + static_cast<size_t>(b) * kXpWarps;
@@ -866,7 +894,13 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
       }
       for (int k = 0; k < G * kXpWarps; ++k)
         pl.xs_pcg_max_steps = std::max(pl.xs_pcg_max_steps, pl.xs_pcg_warp_step[k + 1] - pl.xs_pcg_warp_step[k]);
-      pl.xs_pcg_smem = xs_pcg_smem_bytes(pl.xs_pcg_max_blocks, pl.xs_pcg_max_cams);
+      // the T slots of the owned columns are staged in what shared memory is left, up to the most any CTA has; a CTA
+      // with more sums its columns from T in L2
+      const size_t base = xs_pcg_smem_bytes(pl.xs_pcg_max_blocks, pl.xs_pcg_max_cams, pl.xs_pcg_max_foreign, pl.xs_pcg_max_cta_steps, 0);
+      const size_t room = lim.smem_optin > base + 1024 ? lim.smem_optin - base - 1024 : 0;
+      pl.xs_pcg_stage_slots = static_cast<int>(std::min<size_t>(pl.xs_pcg_max_slots, room / (9 * sizeof(double))));
+      pl.xs_pcg_smem = xs_pcg_smem_bytes(pl.xs_pcg_max_blocks, pl.xs_pcg_max_cams, pl.xs_pcg_max_foreign, pl.xs_pcg_max_cta_steps,
+                                         pl.xs_pcg_stage_slots);
       if (pl.xs_pcg_smem + 1024 > lim.smem_optin) pl.xs_pcg_why = "largest CTA's shared memory exceeds the limit";
       else if (lim.xs_pcg_ctas_per_sm < 1) pl.xs_pcg_why = "no CTA of the kernel fits an SM";
       else if (knobs.xs_resident == 0) pl.xs_pcg_why = "B200_XS_RESIDENT=0";
@@ -937,10 +971,11 @@ inline void print_plan(const KernelPlan& pl, int C, int P, int N, int world, con
       const double share = 648.0 * pl.xs_pcg_max_blocks / 1024.0, limit = static_cast<double>(lim.smem_optin) / 1024.0;
       const double cta = static_cast<double>(pl.xs_pcg_smem) / 1024.0;
       if (pl.xs_pcg)
-        fprintf(stderr, "[b200ba] S PCG: resident, %d CTAs, largest S share %.2f KiB of %.2f KiB (%.2f KiB with M^-1 and vectors), %d warps, at most %d steps per warp\n",
-                lim.sm_count, share, limit, cta, lim.sm_count * kXpWarps, pl.xs_pcg_max_steps);
+        fprintf(stderr, "[b200ba] S PCG: resident, %d CTAs, largest S share %.2f KiB of %.2f KiB (%.2f KiB with M^-1, vectors and staging), %d warps, at most %d steps per warp, at most %d foreign columns, at most %d column slots per CTA (%d staged)\n",
+                lim.sm_count, share, limit, cta, lim.sm_count * kXpWarps, pl.xs_pcg_max_steps, pl.xs_pcg_max_foreign, pl.xs_pcg_max_slots,
+                pl.xs_pcg_stage_slots);
       else
-        fprintf(stderr, "[b200ba] S PCG: two-kernel (%s: largest S share %.2f KiB, %.2f KiB with M^-1 and vectors, of %.2f KiB)\n",
+        fprintf(stderr, "[b200ba] S PCG: two-kernel (%s: largest S share %.2f KiB, %.2f KiB with M^-1, vectors and staging, of %.2f KiB)\n",
                 pl.xs_pcg_why, share, cta, limit);
     }
   } else

@@ -10,14 +10,21 @@
 //   ---- grid barrier ----
 //   tests    the reference's termination and failure tests (cg_alpha, cg_phase_c) on identical fixed-order totals in
 //            every CTA, beta, and the new p of the owned cameras.
-// The product reads p_j of every column j its blocks touch.  A foreign column's p_j is not read back from its owner (that
-// would need a third barrier): the CTA forms it itself from z_j and the previous p_j (cg_next_p, the owner's expression,
-// so the bits agree).  p is double-buffered by iteration parity for that.  A residual reset adds a barrier, the product on
-// x and a second barrier, as CG_RESET_FIRST / CG_RESET_SECOND of the two-kernel loop do.  Every branch around a barrier
-// is taken by the whole grid: it depends only on the iteration count and on totals every CTA sums in the same order.
-// Everything another CTA wrote during the launch (z, p, x, T, red) is read with ld.global.cg.  No atomics: the solve is
-// deterministic given its inputs, and S q equals xs_mul_kernel + xs_col_sum bit for bit; only the grouping of the dot
-// products differs from the two-kernel loop.
+// The product reads p_j of every column j its blocks touch.  A foreign column's p_j (j past the CTA's last row; only the
+// upper triangle is stored) is not read back from its owner (that would need a third barrier): the CTA forms it itself
+// from z_j and the previous p_j (cg_next_p, the owner's expression, so the bits agree), p double-buffered by iteration
+// parity for that.  It does so for all its foreign columns at once, in the same pass that forms the owned cameras' new p,
+// into a shared buffer: the walk then reads every x_j from shared memory, through the plan's CTA-local column index of
+// each block ([owned cameras | foreign columns]), and its steps and column entries from copies the prologue makes, so
+// it reads nothing from global memory.  Likewise the vector phase first copies the T slots of the owned
+// columns (one contiguous range of T) into shared memory in one coalesced pass and sums each column from that copy, in
+// every CTA whose slots fit the room the plan left (stage_slots); any other CTA sums from T in L2, in the same order.  A
+// residual reset adds a barrier, the product on x (its foreign x_j gathered into the same buffer) and a second barrier,
+// as CG_RESET_FIRST / CG_RESET_SECOND of the two-kernel loop do.  Every branch around a barrier is taken by the whole
+// grid: it depends only on the iteration count and on totals every CTA sums in the same order.  Everything another CTA
+// wrote during the launch (z, p, x, T, red) is read with ld.global.cg.  No atomics: the solve is deterministic given its
+// inputs, and S q equals xs_mul_kernel + xs_col_sum bit for bit; only the grouping of the dot products differs from the
+// two-kernel loop.
 #pragma once
 #include "cg_kernel.cuh"
 
@@ -25,18 +32,28 @@ namespace b200 {
 
 constexpr int kXpThreads = 512;
 constexpr int kXpWarps = kXpThreads / 32;
-// dynamic shared memory per CTA: S blocks, M^-1 blocks, and seven vectors (x r p b D_f a z) of the owned cameras
-inline size_t xs_pcg_smem_bytes(int max_blocks, int max_cams) {
-  return sizeof(double) * (81 * static_cast<size_t>(max_blocks) + (81 + 7 * 9) * static_cast<size_t>(max_cams));
+// dynamic shared memory per CTA: S blocks, M^-1 blocks, seven vectors (x r p b D_f a z) of the owned cameras, the
+// product's input [owned cameras | foreign columns], `slots` staged T slots; the product's steps and its blocks' column
+// entries (int2); then the owned columns' col_ptr and the foreign columns' ids
+inline size_t xs_pcg_smem_bytes(int max_blocks, int max_cams, int max_foreign, int max_steps, int slots) {
+  return sizeof(double) * (81 * static_cast<size_t>(max_blocks) + (81 + 7 * 9) * static_cast<size_t>(max_cams) +
+                           9 * static_cast<size_t>(max_cams + max_foreign) + 9 * static_cast<size_t>(slots)) +
+         sizeof(int2) * (static_cast<size_t>(max_steps) + static_cast<size_t>(max_blocks)) +
+         sizeof(int) * (static_cast<size_t>(max_cams) + 1 + static_cast<size_t>(max_foreign));
 }
 
 struct XsPcgArgs {
-  XsView v;
+  XsView v;                   // v.cols: {CTA-local column, T slot} of every block (KernelPlan::xs_pcg_cols)
   CgParams prm;
   int reset;                  // residual reset period (iterations)
   const int2* cta;            // [grid + 1] {first block row, first block} of each CTA
   const int* warp_step;       // [grid * kXpWarps + 1] first product step of each warp
-  int max_blocks, max_cams;   // the shared-memory geometry: the largest CTA's blocks and cameras
+  const int* fptr;            // [grid + 1] each CTA's foreign columns in fcol
+  const int* fcol;            // the foreign columns of each CTA, ascending
+  int max_blocks, max_cams;   // the shared-memory geometry: the largest CTA's blocks and cameras,
+  int max_foreign;            // ... the most foreign columns of a CTA
+  int max_steps;              // ... and the most product steps of a CTA
+  int stage_slots;            // a CTA whose owned columns have at most this many T slots sums them from shared memory
   const double* minv;         // [C][81] M^-1
   const double* rhs;          // [9C]
   const double* Df;           // [9C] or null
@@ -71,6 +88,7 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
   extern __shared__ double smem[];
   __shared__ double scratch[kXpWarps][3];
   __shared__ double s_tot[4];
+  __shared__ int s_nfe;   // entries of the foreign columns (kept here: the product's walk needs every register)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int e = lane / 9, w = lane - 9 * (lane / 9);   // e == 3: lanes 27..31, no block
   const int2 lo = a.cta[blockIdx.x], hi = a.cta[blockIdx.x + 1];
@@ -84,7 +102,17 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
   double* s_d = s_b + 9 * a.max_cams;
   double* s_a = s_d + 9 * a.max_cams;
   double* s_z = s_a + 9 * a.max_cams;
+  double* s_v = s_z + 9 * a.max_cams;                           // the product's input x_l at 9 l: [owned | foreign]
+  double* s_T = s_v + 9 * (a.max_cams + a.max_foreign);         // T slots of the owned columns, from slot s_cp[0] on
+  int2* s_steps = reinterpret_cast<int2*>(s_T + 9 * a.stage_slots);  // the CTA's product steps
+  int2* s_cols = s_steps + a.max_steps;                               // column entries of its blocks
+  int* s_cp = reinterpret_cast<int*>(s_cols + a.max_blocks);          // col_ptr[r0 .. r0 + ncam]
+  int* s_fc = s_cp + a.max_cams + 1;                            // the foreign columns
   const XsView& v = a.v;
+  const int kc = __ldg(a.warp_step + blockIdx.x * kXpWarps);   // the CTA's first step
+  XsView vs = v;                                                // the walk's view: steps and column entries staged
+  vs.steps = s_steps - kc;
+  vs.cols = s_cols - b0;
   const size_t o0 = 9 * static_cast<size_t>(r0);   // first owned entry
   const bool writer = blockIdx.x == 0 && tid == 0;
   const int k0 = __ldg(a.warp_step + blockIdx.x * kXpWarps + warp), k1 = __ldg(a.warp_step + blockIdx.x * kXpWarps + warp + 1);
@@ -103,6 +131,13 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
     }
     for (; i < n; i += kXpThreads) s_S[i] = __ldcg(src + i);
     for (int k = tid; k < 81 * ncam; k += kXpThreads) s_minv[k] = __ldcg(a.minv + 81 * static_cast<size_t>(r0) + k);
+    for (int k = tid; k <= ncam; k += kXpThreads) s_cp[k] = __ldg(v.col_ptr + r0 + k);
+    const int nsteps = __ldg(a.warp_step + (blockIdx.x + 1) * kXpWarps) - kc;
+    for (int k = tid; k < nsteps; k += kXpThreads) s_steps[k] = __ldg(v.steps + kc + k);
+    for (int k = tid; k < nblk; k += kXpThreads) s_cols[k] = __ldg(v.cols + b0 + k);
+    const int f0 = __ldg(a.fptr + blockIdx.x), nf = __ldg(a.fptr + blockIdx.x + 1) - f0;
+    for (int k = tid; k < nf; k += kXpThreads) s_fc[k] = __ldg(a.fcol + f0 + k);
+    if (tid == 0) s_nfe = 9 * nf;
   }
   for (int k = tid; k < nent; k += kXpThreads) {
     s_b[k] = a.rhs[o0 + k];
@@ -116,6 +151,29 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
     for (int u = 0; u < 9; ++u) s[u] = in ? sb[9 * u] : 0.0;
   };
   auto keep_row = [&](int i, int u, double av, double) { s_a[9 * (i - r0) + u] = av; };
+  // the owned columns' T slots into s_T, one coalesced pass (made visible by the caller's next __syncthreads), if they fit
+  auto staged = [&]() { return s_cp[ncam] - s_cp[0] <= a.stage_slots; };
+  auto stage_T = [&]() {
+    if (!staged()) return;
+    const int c0 = s_cp[0];
+    const double* src = v.T + 9 * static_cast<size_t>(c0);
+    const int n = 9 * (s_cp[ncam] - c0);
+    int i = tid;
+    for (; i + 7 * kXpThreads < n; i += 8 * kXpThreads) {
+      double t[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) t[k] = __ldcg(src + i + k * kXpThreads);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) s_T[i + k * kXpThreads] = t[k];
+    }
+    for (; i < n; i += kXpThreads) s_T[i] = __ldcg(src + i);
+  };
+  // q_k = init + the column part of owned entry k, from s_T or else from T (the same sum in the same order)
+  auto col_sum = [&](bool from_s, int k, double init) {
+    const int cl = k / 9;
+    return from_s ? xs_col_sum<true>(s_T, s_cp[0], s_cp[cl], s_cp[cl + 1], k - 9 * cl, init)
+                  : xs_col_sum(v.col_ptr, v.T, static_cast<int>(o0) + k, init);
+  };
   // z = M^-1 r of the owned cameras (s_r complete), and the partials x.(b+r), r.r, r.z into red[CTA][1..3]
   auto precondition = [&]() {
     __syncthreads();
@@ -159,30 +217,30 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
   rho = tot[2];
 
   for (;;) {
-    // ---- p of iteration it + 1 on the owned cameras; its share of D_f^2 p.p
+    // ---- p of iteration it + 1: the owned cameras' (and their share of D_f^2 p.p), and in the threads past them the
+    // foreign columns', from z and p of iteration it
     double pq = 0.0;
-    for (int k = tid; k < nent; k += kXpThreads) {
-      const double pn = cg_next_p(it, s_z[k], beta, s_p[k]);
-      s_p[k] = pn;
-      a.p[(it + 1) & 1][o0 + k] = pn;
-      pq += s_d[k] * s_d[k] * pn * pn;
+    const double* p_prev = a.p[it & 1];
+    for (int k = tid; k < nent + s_nfe; k += kXpThreads) {
+      if (k < nent) {
+        const double pn = cg_next_p(it, s_z[k], beta, s_p[k]);
+        s_p[k] = pn;
+        s_v[k] = pn;
+        a.p[(it + 1) & 1][o0 + k] = pn;
+        pq += s_d[k] * s_d[k] * pn * pn;
+      } else {
+        const int fl = (k - nent) / 9;
+        const size_t o = 9 * static_cast<size_t>(s_fc[fl]) + (k - nent - 9 * fl);
+        s_v[k] = cg_next_p(it, __ldcg(a.z + o), beta, __ldcg(p_prev + o));
+      }
     }
-    const double* p_prev = a.p[it & 1];   // p of iteration it, for the foreign columns
     ++it;
     __syncthreads();
     // ---- product S p
     {
       XsWalk wk;
-      xs_walk_begin(v, k0, k1, e, w, load_s, wk);
-      pq += xs_walk(
-          v, k0, k1, lane, e, w, load_s,
-          [&](int j, int w) -> double {
-            const int l = j - r0;
-            if (l >= 0 && l < ncam) return s_p[9 * l + w];
-            const size_t o = 9 * static_cast<size_t>(j) + w;
-            return cg_next_p(it - 1, __ldcg(a.z + o), beta, __ldcg(p_prev + o));
-          },
-          keep_row, wk);
+      xs_walk_begin<true>(vs, k0, k1, e, w, load_s, wk);
+      pq += xs_walk<true>(vs, k0, k1, lane, e, w, load_s, [&](int l, int w) { return s_v[9 * l + w]; }, keep_row, wk);
     }
     {
       double d1 = 0.0, d2 = 0.0;
@@ -192,39 +250,48 @@ __global__ void __launch_bounds__(kXpThreads, 1) xs_pcg_kernel(XsPcgArgs a) {
     XP_STAMP(1);
     grid.sync();
     XP_STAMP(2);
-    // ---- vector phase
+    // ---- vector phase (cg_totals' __syncthreads make the staged T visible)
     double pq_tot, alpha = 0.0;
+    const bool reset = it % a.reset == 0;
+    if (!reset) stage_T();
     cg_totals(a.red, gridDim.x, 0, 1, &pq_tot, s_tot);
     if (!cg_alpha(pq_tot, rho, it, a.st, writer, &alpha)) return;
-    const bool reset = it % a.reset == 0;
+    const bool from_s = staged();
     for (int k = tid; k < nent; k += kXpThreads) {
       const double pj = s_p[k];
       double xj = s_x[k];
       xj += alpha * pj;
       s_x[k] = xj;
       a.x[o0 + k] = xj;
-      if (!reset) {
+      if (reset) {
+        s_v[k] = xj;
+      } else {
         const double dj = s_d[k];
-        const double q = xs_col_sum(v.col_ptr, v.T, static_cast<int>(o0) + k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), pj)));
+        const double q = col_sum(from_s, k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), pj)));
         double rj = s_r[k];
         rj -= alpha * q;
         s_r[k] = rj;
       }
     }
     if (reset) {
-      // r = b - S x: the product on x, whose every column is read back from its owner
+      // r = b - S x: the product on x, its foreign columns read back from their owners
       grid.sync();
+      for (int k = tid; k < s_nfe; k += kXpThreads) {
+        const int fl = k / 9;
+        s_v[nent + k] = __ldcg(a.x + 9 * static_cast<size_t>(s_fc[fl]) + (k - 9 * fl));
+      }
+      __syncthreads();
       {
         XsWalk wk;
-        xs_walk_begin(v, k0, k1, e, w, load_s, wk);
-        xs_walk(
-            v, k0, k1, lane, e, w, load_s, [&](int j, int w) { return __ldcg(a.x + 9 * static_cast<size_t>(j) + w); },
-            keep_row, wk);
+        xs_walk_begin<true>(vs, k0, k1, e, w, load_s, wk);
+        xs_walk<true>(vs, k0, k1, lane, e, w, load_s, [&](int l, int w) { return s_v[9 * l + w]; }, keep_row, wk);
       }
       grid.sync();
+      stage_T();
+      __syncthreads();
       for (int k = tid; k < nent; k += kXpThreads) {
         const double dj = s_d[k];
-        const double q = xs_col_sum(v.col_ptr, v.T, static_cast<int>(o0) + k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), s_x[k])));
+        const double q = col_sum(from_s, k, __dadd_rn(s_a[k], __dmul_rn(__dmul_rn(dj, dj), s_x[k])));
         s_r[k] = s_b[k] - q;
       }
     }
