@@ -23,6 +23,8 @@ ERR_UNSUPPORTED = -6
 LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR = 0, 1, 2, 3
 PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION = 0, 1, 2, 3
 ITERATIVE_SCHUR, DENSE_SCHUR, SPARSE_SCHUR = 0, 1, 2
+LEVENBERG_MARQUARDT, DOGLEG = 0, 1                  # trust_region_strategy_type
+TRADITIONAL_DOGLEG, SUBSPACE_DOGLEG = 0, 1          # dogleg_type
 # b200_plan_sparse_schur's statistics (B200_SPARSE_STAT_*), in order
 SPARSE_STATS = ("s_blocks", "l_blocks", "l_blocks_caller", "l_blocks_min_degree", "flops_caller", "flops_min_degree",
                 "supernodes", "tree_height", "order", "factor_bytes")
@@ -61,7 +63,7 @@ class LmOptions(C.Structure):
                 ("min_trust_region_radius", C.c_double), ("min_relative_decrease", C.c_double),
                 ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
-                ("linear_solver", SolverOptions)]
+                ("linear_solver", SolverOptions), ("trust_region_strategy_type", C.c_int32), ("dogleg_type", C.c_int32)]
 
 
 class LmIteration(C.Structure):

@@ -437,6 +437,86 @@ __global__ void __launch_bounds__(kTile) model_cost_kernel(ProblemView p, const 
   }
 }
 
+// DOGLEG's one pass over J per Gauss-Newton step (dogleg_strategy.cc:185-194, :699-714): with a = g / diagonal and
+// b = gn / diagonal, the per-tile partials of |J a|^2 and, when gn != nullptr, of |J b|^2 and (J a).(J b), stored at
+// partial[k * num_tiles + tile] and reduced in fixed order afterwards.
+__global__ void __launch_bounds__(kTile) dogleg_gram_kernel(ProblemView p, const double* __restrict__ g,
+                                                            const double* __restrict__ gn,
+                                                            const double* __restrict__ diagonal, double* partial) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const TileSmem s = carve_smem<1, 1>(smem_raw);
+  tile_prologue(s);
+  const int tid = threadIdx.x;
+  const bool two = gn != nullptr;
+  uint32_t parity = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const TileDesc d = p.tiles[tile];
+    tile_begin(p, d, s, true, true);
+    double ac[9], ap[3], bc[9], bp[3];
+    const bool active = tid < d.obs_count;
+    if (active) {
+      const size_t oc = 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(s.sCam[tid]);
+      const size_t op = 3 * static_cast<size_t>(d.pt_begin + s.sSlotPt[tid]);
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        const double dk = diagonal[oc + k];
+        ac[k] = g[oc + k] / dk;
+        bc[k] = two ? gn[oc + k] / dk : 0.0;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double dk = diagonal[op + k];
+        ap[k] = g[op + k] / dk;
+        bp[k] = two ? gn[op + k] / dk : 0.0;
+      }
+    }
+    mbar_wait(s.bar, parity);
+    parity ^= 1;
+    double aa = 0.0, bb = 0.0, ab = 0.0;
+    if (active) {
+      const double* e = s.sE + tid * 6;
+      const double2 e0 = lds2(e), e1 = lds2(e + 2), e2 = lds2(e + 4);
+      const double ev[6] = {e0.x, e0.y, e1.x, e1.y, e2.x, e2.y};
+      double t0 = 0.0, t1 = 0.0, u0 = 0.0, u1 = 0.0;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        t0 += ev[k] * ap[k];
+        t1 += ev[3 + k] * ap[k];
+        u0 += ev[k] * bp[k];
+        u1 += ev[3 + k] * bp[k];
+      }
+      double f[18];
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        const double2 v = lds2(s.sF + tid * 18 + 2 * k);
+        f[2 * k] = v.x;
+        f[2 * k + 1] = v.y;
+      }
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        t0 += f[k] * ac[k];
+        t1 += f[9 + k] * ac[k];
+        u0 += f[k] * bc[k];
+        u1 += f[9 + k] * bc[k];
+      }
+      aa = t0 * t0 + t1 * t1;
+      bb = u0 * u0 + u1 * u1;
+      ab = t0 * u0 + t1 * u1;
+    }
+    const double taa = block_sum<kTile>(aa, s.sPt);
+    if (tid == 0) partial[tile] = taa;
+    if (two) {
+      const double tbb = block_sum<kTile>(bb, s.sPt);
+      const double tab = block_sum<kTile>(ab, s.sPt);
+      if (tid == 0) {
+        partial[static_cast<size_t>(p.num_tiles) + tile] = tbb;
+        partial[2 * static_cast<size_t>(p.num_tiles) + tile] = tab;
+      }
+    }
+    __syncthreads();
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // y += J x  (rows are independent; x = [points | cameras])
 // ------------------------------------------------------------------------------------------------

@@ -57,6 +57,10 @@ enum KernelId {
   K_SCHUR_PCG,
   K_SPARSE_SCATTER,
   K_SPARSE_FACTOR,
+  K_DOGLEG_GRAM,
+  K_DOGLEG_DIAG,
+  K_DOGLEG_GN,
+  K_DOGLEG_STEP,
   K_MISC,
   K_COUNT
 };
@@ -64,7 +68,7 @@ const char* const kKernelNames[K_COUNT] = {"evaluate_jacobian", "evaluate_cost",
                                            "jacobian_multiply", "jacobian_t_multiply", "jtj_multiply", "schur_init",
                                            "schur_multiply", "schur_multiply_big_points", "camera_reduce", "schur_diag_blocks", "invert_9x9", "back_substitute",
                                            "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg",
-                                           "sparse_scatter", "sparse_factor", "misc"};
+                                           "sparse_scatter", "sparse_factor", "dogleg_gram", "dogleg_diagonal", "dogleg_gn", "dogleg_step", "misc"};
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.
@@ -929,6 +933,11 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
   bpo[K_PMV_LEFT_E] = 48 * Nn + 16 * Nn + 4 * Pp + 48 * Pp;             // E cells, y, chunk boundaries, x_e read + written
   bpo[K_PMV_LEFT_F] = 144 * Nn + 16 * Nn + 4 * Nn + 144 * Cc;           // F cells, y, row list, x_f read + written
   bpo[K_MODEL_COST] = 196 * Nn + 16 * Nn + 4 * Pp + 8.0 * (3 * Pp + 9 * Cc);
+  // J, chunk ids, g and the diagonal; the subspace variant also reads gn (b200_lm_solve sets that figure for its run)
+  bpo[K_DOGLEG_GRAM] = 196 * Nn + 4 * Pp + 16.0 * (3 * Pp + 9 * Cc);
+  bpo[K_DOGLEG_DIAG] = 48.0 * (3 * Pp + 9 * Cc);   // refresh: colnorm^2, gradient, scale read; diagonal, g, D written
+  bpo[K_DOGLEG_GN] = 32.0 * (3 * Pp + 9 * Cc);     // y, diagonal, g read; gn written
+  bpo[K_DOGLEG_STEP] = 56.0 * (3 * Pp + 9 * Cc);   // g, gn, diagonal, scale, x read; step, cand written
   if (pl.xs) {   // explicit S: the product and the assembly that replaces the block-diagonal pass
     bpo[K_SCHUR_MUL] = xs_mul_bytes;
     bpo[K_DIAG_BLOCKS] = xs_asm_bytes;

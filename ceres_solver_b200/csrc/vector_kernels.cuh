@@ -127,6 +127,92 @@ __global__ void __launch_bounds__(256) grad_norm_kernel(int n, const double* __r
     partial[blockIdx.x * 2 + 1] = sq;
   }
 }
+// ---------------------------------------------------------------- DOGLEG vector kernels (dogleg_strategy.cc)
+// refresh: diagonal = sqrt(clamp(colnorm^2, min, max)) (:123-128) and g = scale * gradient / diagonal.  The reference
+// forms g as J_s' r / diagonal (:176-181) with J_s the scaled Jacobian; J_s' r = scale * (J' r) up to rounding, and J' r
+// is the gradient the evaluate already wrote, so no pass over J is needed.  Always: D = diagonal * sqrt(mu) (:561).
+__global__ void __launch_bounds__(256) dogleg_diagonal_kernel(int n, int refresh, const double* __restrict__ sqnorm,
+                                                              const double* __restrict__ gradient,
+                                                              const double* __restrict__ scale, double* diagonal,
+                                                              double* g, double* D, double min_d, double max_d,
+                                                              double sqrt_mu) {
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    double d = diagonal[i];
+    if (refresh) {
+      d = sqrt(fmin(fmax(sqnorm[i], min_d), max_d));
+      diagonal[i] = d;
+      g[i] = __dmul_rn(scale[i], gradient[i]) / d;
+    }
+    D[i] = __dmul_rn(d, sqrt_mu);
+  }
+}
+// After a solve J'J + D^2 y = J'r: gn = -diagonal * y (:612); partials {|g|^2, g.gn, |gn|^2, non-finite y count} (:594).
+__global__ void __launch_bounds__(256) dogleg_gn_kernel(int n, const double* __restrict__ y,
+                                                        const double* __restrict__ diagonal,
+                                                        const double* __restrict__ g, double* gn, double* partial) {
+  __shared__ double scratch[32];
+  double a = 0.0, b = 0.0, c = 0.0, bad = 0.0;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const double yi = y[i];
+    const double v = __dmul_rn(yi, -diagonal[i]);
+    gn[i] = v;
+    const double gi = g[i];
+    a = __fma_rn(gi, gi, a);
+    b = __fma_rn(gi, v, b);
+    c = __fma_rn(v, v, c);
+    if (!isfinite(yi)) bad += 1.0;
+  }
+  a = block_sum<256>(a, scratch);
+  b = block_sum<256>(b, scratch);
+  c = block_sum<256>(c, scratch);
+  bad = block_sum<256>(bad, scratch);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x * 4 + 0] = a;
+    partial[blockIdx.x * 4 + 1] = b;
+    partial[blockIdx.x * 4 + 2] = c;
+    partial[blockIdx.x * 4 + 3] = bad;
+  }
+}
+// The dogleg step (dogleg.h StepKind): v = gn (kind 0), cg g (kind 1) or cg g + cn gn (kind 2), selected rather than
+// multiplied by 0; step = v / diagonal; delta = step * scale; cand = x + delta.
+// Partials {|x - cand|^2, |x|^2, non-finite step count, |v|^2 (dogleg_step_norm_ of the interpolation, :251)}.
+__global__ void __launch_bounds__(256)
+    dogleg_step_kernel(int n, int kind, double cg, double cn, const double* __restrict__ g, const double* __restrict__ gn,
+                       const double* __restrict__ diagonal, const double* __restrict__ scale,
+                       const double* __restrict__ x, double* step, double* cand, double* partial) {
+  __shared__ double scratch[32];
+  double a = 0.0, b = 0.0, c = 0.0, e = 0.0;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    double v;
+    if (kind == 0) v = gn[i];
+    else if (kind == 1) v = __dmul_rn(cg, g[i]);
+    else v = __dadd_rn(__dmul_rn(cg, g[i]), __dmul_rn(cn, gn[i]));
+    const double si = v / diagonal[i];
+    step[i] = si;
+    const double xi = x[i];
+    const double ci = __dadd_rn(xi, __dmul_rn(si, scale[i]));
+    cand[i] = ci;
+    const double dd = xi - ci;
+    a = __fma_rn(dd, dd, a);
+    b = __fma_rn(xi, xi, b);
+    if (!isfinite(si)) c += 1.0;
+    e = __fma_rn(v, v, e);
+  }
+  a = block_sum<256>(a, scratch);
+  b = block_sum<256>(b, scratch);
+  c = block_sum<256>(c, scratch);
+  e = block_sum<256>(e, scratch);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x * 4 + 0] = a;
+    partial[blockIdx.x * 4 + 1] = b;
+    partial[blockIdx.x * 4 + 2] = c;
+    partial[blockIdx.x * 4 + 3] = e;
+  }
+}
+
 // out[s] = reduce over blocks of partial[b*slots + s]; op_mask bit s set => max, else sum.
 __global__ void __launch_bounds__(32) reduce_final_kernel(int blocks, int slots, unsigned op_mask,
                                                           const double* __restrict__ partial, double* out) {

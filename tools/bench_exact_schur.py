@@ -1,9 +1,12 @@
 """The two exact LM-step solvers, DENSE_SCHUR (b200_dense_schur_solve: dense S, cuSOLVER Cholesky) and SPARSE_SCHUR
 (b200_sparse_schur_solve: block-sparse S, supernodal Cholesky), on the same handle of each problem: time per solve from a host
-clock around synchronised calls and from the CUDA-event stats of a profiled pass, LM iterations per second of b200_lm_solve
-with each solver type, the symbolic statistics and the host analysis time, and the card's name and power limit.
+clock around synchronised calls and from the CUDA-event stats of a profiled pass; b200_lm_solve with each solver type and each
+trust-region strategy (LM, traditional and subspace DOGLEG): iterations per second, factorisations per iteration, the cost
+after K iterations and the rejected steps; the symbolic statistics and the host analysis time, and the card's name and power
+limit.
 
-    python tools/bench_exact_schur.py [--reps 5] [--lm-iterations 5] [--problems ladybug-1723,...] [--out results.json]
+    python tools/bench_exact_schur.py [--reps 5] [--lm-iterations 5] [--problems ladybug-1723,...]
+                                      [--strategies lm,traditional_dogleg,subspace_dogleg] [--out results.json]
 
 One JSON line per problem on stdout.  Needs an H100; nothing is written unless --out is given.
 """
@@ -53,15 +56,27 @@ def timed_solves(gpu, solve, b, D, reps):
     return x, term, ms, kernels
 
 
-def lm_rate(gpu, state, solver_type, iterations):
-    o = gpu.lm_options(max_num_iterations=iterations)
-    o.linear_solver_type = solver_type
-    gpu.lm_solve(state, gpu.lm_options(max_num_iterations=1, linear_solver_type=solver_type))   # warm-up
+# trust-region strategy axis: (name, trust_region_strategy_type, dogleg_type)
+STRATEGIES = [("lm", cs.LEVENBERG_MARQUARDT, cs.TRADITIONAL_DOGLEG), ("traditional_dogleg", cs.DOGLEG, cs.TRADITIONAL_DOGLEG),
+              ("subspace_dogleg", cs.DOGLEG, cs.SUBSPACE_DOGLEG)]
+
+
+def lm_rate(gpu, state, solver_type, iterations, strategy=cs.LEVENBERG_MARQUARDT, dogleg_type=cs.TRADITIONAL_DOGLEG):
+    """b200_lm_solve for `iterations` iterations: iterations per second, the cost reached, factorisations per iteration
+    (launches of the dense assembly or of the sparse factor kernel: a rejected DOGLEG step reuses its factorisation, a
+    rejected LM step does not) and the rejected and invalid steps of the run."""
+    kw = dict(linear_solver_type=solver_type, trust_region_strategy_type=strategy, dogleg_type=dogleg_type)
+    gpu.lm_solve(state, gpu.lm_options(max_num_iterations=1, **kw))   # warm-up
     gpu.synchronize()
+    gpu.stats_reset()
     t = time.perf_counter()
-    _, recs = gpu.lm_solve(state, o)
+    _, recs = gpu.lm_solve(state, gpu.lm_options(max_num_iterations=iterations, **kw))
     dt = time.perf_counter() - t
-    return (len(recs) - 1) / dt, recs[-1]["cost"]
+    its = len(recs) - 1
+    factor = gpu.stats()["schur_diag_blocks" if solver_type == cs.DENSE_SCHUR else "sparse_factor"]["launches"]
+    return dict(its_per_s=its / dt, cost=recs[-1]["cost"], iterations=its, factorisations_per_iteration=factor / max(its, 1),
+                rejected=sum(1 for r in recs[1:] if r["step_is_valid"] and not r["step_is_successful"]),
+                invalid=sum(1 for r in recs[1:] if not r["step_is_valid"]))
 
 
 def main():
@@ -69,6 +84,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--lm-iterations", type=int, default=5)
     ap.add_argument("--problems", default=",".join(PROBLEMS))
+    ap.add_argument("--strategies", default=",".join(n for n, _, _ in STRATEGIES))
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     device = card()
@@ -91,8 +107,14 @@ def main():
         xd, td, row["dense_ms"], row["dense_kernels_ms"] = timed_solves(gpu, gpu.dense_schur_solve, res, D, a.reps)
         row["terminations"] = [int(ts), int(td)]
         row["relerr_sparse_dense"] = float(np.linalg.norm(xs - xd) / np.linalg.norm(xd))
-        row["lm_its_per_s_sparse"], row["lm_cost_sparse"] = lm_rate(gpu, state, cs.SPARSE_SCHUR, a.lm_iterations)
-        row["lm_its_per_s_dense"], row["lm_cost_dense"] = lm_rate(gpu, state, cs.DENSE_SCHUR, a.lm_iterations)
+        for sname, solver in (("sparse", cs.SPARSE_SCHUR), ("dense", cs.DENSE_SCHUR)):
+            for name_s, strategy, dogleg_type in STRATEGIES:
+                if name_s not in a.strategies.split(","):
+                    continue
+                rate = lm_rate(gpu, state, solver, a.lm_iterations, strategy, dogleg_type)
+                if name_s == "lm":
+                    row["lm_its_per_s_" + sname], row["lm_cost_" + sname] = rate["its_per_s"], rate["cost"]
+                row.setdefault("strategies", {})["%s/%s" % (name_s, sname)] = rate
         gpu.close()
         print(json.dumps(row), flush=True)
         results.append(row)
