@@ -196,6 +196,9 @@ __device__ __forceinline__ void xs_step_s(const XsView& v, int2 d, int e, int w,
 // takes the row part of row i in lanes 0..8.  xs_walk_begin loads what does not depend on x (before a grid dependency
 // resolves); xs_walk returns the lane's share of x . S x (x_i . a_i over its rows, x_j . t_ij over its blocks).
 // kShared: the descriptors and column entries come from shared memory (xs_step_desc).
+// A range may begin or end inside a row (the resident PCG splits long rows over warps): a range that begins inside row
+// i reads x_i with load_xi(i, u) instead of from its diagonal block, and one that ends inside a row passes row_out the
+// sum of that row's blocks in the range.  Either way x_i . (that sum) goes into the returned share.
 struct XsWalk {
   XsStepData nx;   // step k + 1
   int2 d2, c2;     // step k + 2: descriptor and column entry
@@ -208,15 +211,19 @@ __device__ __forceinline__ void xs_walk_begin(const XsView& v, int k0, int k1, i
   wk.d2 = xs_step_desc<kShared>(v, k0 + 1, k1);
   wk.c2 = xs_step_col<kShared>(v, wk.d2, e);
 }
-template <bool kShared = false, class LoadS, class LoadX, class RowOut>
+constexpr int kXsStepRowMask = (1 << kXsStepCountShift) - 1;
+template <bool kShared = false, class LoadS, class LoadX, class LoadXi, class RowOut>
 __device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int lane, int e, int w, LoadS load_s, LoadX load_x,
-                                          RowOut row_out, XsWalk& wk) {
+                                          LoadXi load_xi, RowOut row_out, XsWalk& wk) {
   XsStepData& nx = wk.nx;
   int2 d2 = wk.d2, c2 = wk.c2;
   double nx_x = xs_lane_in(nx.d, e) ? load_x(nx.c.x, w) : 0.0;
   double acc[9], xi[9];
 #pragma unroll
   for (int u = 0; u < 9; ++u) acc[u] = xi[u] = 0.0;
+  if (k0 < k1 && !(nx.d.y & kXsStepFirst))
+#pragma unroll
+    for (int u = 0; u < 9; ++u) xi[u] = load_xi(nx.d.y & kXsStepRowMask, u);
   double pq = 0.0;
   for (int k = k0; k < k1; ++k) {
     const int2 d = nx.d, c = nx.c;
@@ -245,7 +252,7 @@ __device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int l
       v.T[9 * static_cast<size_t>(c.y) + w] = t;
       pq += xj * t;
     }
-    if (d.y & kXsStepLast) {
+    if ((d.y & kXsStepLast) || k + 1 == k1) {
       // a_i[u] = sum over the lanes of acc[u]: a butterfly, so every lane holds the same bits
       double mine = 0.0, xo = 0.0;
 #pragma unroll
@@ -261,7 +268,7 @@ __device__ __forceinline__ double xs_walk(const XsView& v, int k0, int k1, int l
       }
       if (lane < 9) {
         pq += xo * mine;
-        row_out(d.y & ((1 << kXsStepCountShift) - 1), lane, mine, xo);
+        row_out(d.y & kXsStepRowMask, lane, mine, xo);
       }
     }
   }
@@ -286,8 +293,9 @@ __global__ void __launch_bounds__(kXsThreads, kXsMinCtas) xs_mul_kernel(XsView v
   xs_walk_begin(v, k0, k1, e, w, load_s, wk);
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (done_flag != nullptr && __ldcg(done_flag) != 0) return;
+  auto load_x = [&](int j, int w) { return __ldcg(x + 9 * static_cast<size_t>(j) + w); };
   double pq = xs_walk(
-      v, k0, k1, lane, e, w, load_s, [&](int j, int w) { return __ldcg(x + 9 * static_cast<size_t>(j) + w); },
+      v, k0, k1, lane, e, w, load_s, load_x, load_x,
       [&](int i, int u, double a, double xo) {
         const size_t o = 9 * static_cast<size_t>(i) + u;
         double out = a;

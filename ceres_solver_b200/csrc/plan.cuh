@@ -207,6 +207,8 @@ struct KernelPlan {
                                        // else foreign column l - n of the block's CTA
   int xs_pcg_max_blocks = 0, xs_pcg_max_cams = 0, xs_pcg_max_steps = 0, xs_pcg_max_foreign = 0;
   int xs_pcg_max_cta_steps = 0;        // the most product steps of a CTA
+  int xs_pcg_walk_max = 0;             // the most steps of a warp, counting one per row segment for its sum
+  int xs_pcg_split_rows = 0;           // rows whose steps are cut over two or more warps, all CTAs together
   int xs_pcg_max_slots = 0;            // the most T slots of a CTA's owned columns
   int xs_pcg_stage_slots = 0;          // ... that fit the shared memory left: a CTA with at most these stages them
   size_t xs_pcg_smem = 0;
@@ -823,8 +825,8 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
     for (int k = 0; k < nw; ++k) pl.xs_max_steps = std::max(pl.xs_max_steps, pl.xs_warp_step[k + 1] - pl.xs_warp_step[k]);
     // Resident PCG (xs_pcg.cuh): the block rows in G contiguous ranges with the smallest possible largest range in blocks
     // (the share of S a CTA holds in shared memory): the least capacity K at which filling the CTAs in row order, each up
-    // to K blocks, needs at most G of them.  Within a CTA its rows go to the warps balanced by steps plus one per row, as
-    // above.  Every CTA also gets the sorted list of its foreign columns (j past its last row: its blocks are in the upper
+    // to K blocks, needs at most G of them.  Within a CTA its steps go to the warps in contiguous
+    // ranges that may cut rows (below).  Every CTA also gets the sorted list of its foreign columns (j past its last row: its blocks are in the upper
     // triangle, so j below that is an owned camera) and every block its column as an index into [owned cameras | foreign
     // columns].  Resident when the largest CTA's blocks (with their column entries), M^-1 blocks and vectors, the most
     // foreign columns and the most product steps of a CTA fit one CTA's shared memory next to the static scratch, and
@@ -884,17 +886,44 @@ inline void plan_kernels(int C, int P, int N, const int* caller_cam, const doubl
         pl.xs_pcg_fcol.insert(pl.xs_pcg_fcol.end(), fc.begin(), fc.end());
         pl.xs_pcg_fptr[b + 1] = static_cast<int>(pl.xs_pcg_fcol.size());
         pl.xs_pcg_max_foreign = std::max(pl.xs_pcg_max_foreign, static_cast<int>(fc.size()));
-        double tot = 0.0, cum = 0.0;
-        for (int i = i0; i < i1; ++i) tot += row_steps(i) + 1;
-        int* ws = pl.xs_pcg_warp_step.data() + static_cast<size_t>(b) * kXpWarps;
-        int wv = 0;
-        ws[0] = first_step[i0];
-        for (int i = i0; i < i1; ++i) {
-          const int owner = std::min(kXpWarps - 1, static_cast<int>(cum * kXpWarps / tot));
-          while (wv < owner) ws[++wv] = first_step[i];
-          cum += row_steps(i) + 1;
+        // the CTA's steps in kXpWarps contiguous ranges, cut anywhere, with the least largest cost: a range costs its steps
+        // plus one per row segment in it (the segment's butterfly).  Filling the warps in order, each up to K, is optimal
+        // for a given K (extending a range never lowers its cost); K is the least that needs at most kXpWarps of them.
+        const int s0 = first_step[i0], s1 = first_step[i1];
+        auto fill = [&](int K, int* ws) {
+          int g = 0, cost = 0;
+          if (ws != nullptr) ws[0] = s0;
+          for (int k = s0; k < s1; ++k) {
+            const bool row_start = (pl.xs_steps[k].y & kXsStepFirst) != 0;
+            if (cost + 1 + (row_start || cost == 0) > K) {
+              if (++g == kXpWarps) return g + 1;
+              if (ws != nullptr) ws[g] = k;
+              cost = 0;
+            }
+            cost += 1 + (row_start || cost == 0);
+          }
+          if (ws != nullptr)
+            while (g < kXpWarps - 1) ws[++g] = s1;
+          return g + 1;
+        };
+        int klo = 2, khi = std::max(2, 2 * (s1 - s0));
+        while (klo < khi) {
+          const int mid = klo + (khi - klo) / 2;
+          if (fill(mid, nullptr) <= kXpWarps) khi = mid;
+          else klo = mid + 1;
         }
-        while (wv < kXpWarps - 1) ws[++wv] = first_step[i1];
+        int* ws = pl.xs_pcg_warp_step.data() + static_cast<size_t>(b) * kXpWarps;
+        fill(klo, ws);
+        for (int wv = 0; wv < kXpWarps; ++wv) {
+          const int ka = ws[wv], kb = wv + 1 < kXpWarps ? ws[wv + 1] : s1;   // ws[kXpWarps]: the next CTA's, not set yet
+          if (ka == kb) continue;
+          int cost = kb - ka + 1;
+          for (int k = ka + 1; k < kb; ++k) cost += (pl.xs_steps[k].y & kXsStepFirst) != 0;
+          pl.xs_pcg_walk_max = std::max(pl.xs_pcg_walk_max, cost);
+          const int df = pl.xs_steps[ka].y, dl = pl.xs_steps[kb - 1].y;
+          // the range ends inside a row that begins in it
+          if (!(dl & kXsStepLast) && ((df & kXsStepFirst) || (df & kXsStepRowMask) != (dl & kXsStepRowMask))) ++pl.xs_pcg_split_rows;
+        }
       }
       for (int k = 0; k < G * kXpWarps; ++k)
         pl.xs_pcg_max_steps = std::max(pl.xs_pcg_max_steps, pl.xs_pcg_warp_step[k + 1] - pl.xs_pcg_warp_step[k]);
@@ -979,13 +1008,16 @@ inline void print_plan(const KernelPlan& pl, int C, int P, int N, int world, con
     if (pl.xs) {
       const double share = 648.0 * pl.xs_pcg_max_blocks / 1024.0, limit = static_cast<double>(lim.smem_optin) / 1024.0;
       const double cta = static_cast<double>(pl.xs_pcg_smem) / 1024.0;
-      if (pl.xs_pcg)
+      if (pl.xs_pcg) {
         fprintf(stderr, "[b200ba] S PCG: resident, %d CTAs, largest S share %.2f KiB of %.2f KiB (%.2f KiB with M^-1, vectors and staging), %d warps, at most %d steps per warp, at most %d foreign columns, at most %d column slots per CTA (%d staged)\n",
                 lim.sm_count, share, limit, cta, lim.sm_count * kXpWarps, pl.xs_pcg_max_steps, pl.xs_pcg_max_foreign, pl.xs_pcg_max_slots,
                 pl.xs_pcg_stage_slots);
-      else
+        fprintf(stderr, "[b200ba] S PCG walk: at most %d steps per warp (one per row segment included), %d split rows\n",
+                pl.xs_pcg_walk_max, pl.xs_pcg_split_rows);
+      } else {
         fprintf(stderr, "[b200ba] S PCG: two-kernel (%s: largest S share %.2f KiB, %.2f KiB with M^-1, vectors and staging, of %.2f KiB)\n",
                 pl.xs_pcg_why, share, cta, limit);
+      }
     }
   } else
     fprintf(stderr, "[b200ba] S plan: implicit, sharded\n");
