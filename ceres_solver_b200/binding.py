@@ -63,7 +63,8 @@ class LmOptions(C.Structure):
                 ("min_trust_region_radius", C.c_double), ("min_relative_decrease", C.c_double),
                 ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
-                ("linear_solver", SolverOptions), ("trust_region_strategy_type", C.c_int32), ("dogleg_type", C.c_int32)]
+                ("linear_solver", SolverOptions), ("trust_region_strategy_type", C.c_int32), ("dogleg_type", C.c_int32),
+                ("use_mixed_precision_solves", C.c_int32), ("max_num_refinement_iterations", C.c_int32)]
 
 
 class LmIteration(C.Structure):
@@ -85,7 +86,7 @@ SYMBOLS = [
     "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
-    "b200_schur_solve", "b200_dense_schur_solve", "b200_schur_init", "b200_schur_rhs", "b200_schur_ete_inverse", "b200_schur_multiply",
+    "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options", "b200_schur_init", "b200_schur_rhs", "b200_schur_ete_inverse", "b200_schur_multiply",
     "b200_schur_back_substitute", "b200_schur_jacobi_update", "b200_block_jacobi_update",
     "b200_lm_options_default", "b200_lm_solve", "b200_profile_enable", "b200_stats_reset", "b200_stats_get",
     "b200_total_launches", "b200_synchronize", "b200_transfer_bytes",
@@ -286,6 +287,11 @@ class Problem:
         bp = _d(_f64(b)) if b is not None else None
         _check(lib().b200_sparse_schur_solve(self.h, bp, _d(_f64(D)), _d(x), C.byref(s)))
         return x, s.num_iterations, s.termination_type
+
+    def set_exact_solve_options(self, use_mixed_precision_solves=False, max_num_refinement_iterations=0):
+        """LinearSolver::Options::use_mixed_precision_solves / max_num_refinement_iterations of the later dense and sparse
+        Schur solves on this handle."""
+        _check(lib().b200_set_exact_solve_options(self.h, int(use_mixed_precision_solves), int(max_num_refinement_iterations)))
 
     def model_cost_change(self, step):
         out = C.c_double(0.0)

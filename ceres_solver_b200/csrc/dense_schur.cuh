@@ -110,4 +110,37 @@ __global__ void __launch_bounds__(256) dense_schur_diagonal_kernel(int n, const 
   if (j < n && Df != nullptr) A[j + static_cast<size_t>(j) * lda] += Df[j] * Df[j];
 }
 
+// Iterative refinement of the exact solves (RefinedSparseCholesky::Solve sparse_cholesky.cc:160-170, RefinedDenseCholesky::
+// Solve dense_cholesky.cc:337-349): x_f = solve(rhs_S), then k times r = rhs_S - (S + D_f^2) x_f in FP64 and x_f += solve(r).
+// A solve's vector v is indexed by position pos(k) = 9 pinv[k / 9] + k % 9 (the sparse factor's elimination order) or, with
+// pinv == NULL, by k itself (the dense factor).
+
+// v[pos(k)] <- rhs[k] - Sx[k] (Sx may be NULL), rounded to T once.
+template <typename T>
+__global__ void __launch_bounds__(256) refine_residual_kernel(int n, const int* __restrict__ pinv, const double* __restrict__ rhs,
+                                                             const double* __restrict__ Sx, T* __restrict__ v) {
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    v[pinv != nullptr ? 9 * pinv[k / 9] + k % 9 : k] = static_cast<T>(Sx != nullptr ? rhs[k] - Sx[k] : rhs[k]);
+}
+
+// x[k] <- (add ? x[k] : 0) + v[pos(k)] widened to double.
+template <typename T>
+__global__ void __launch_bounds__(256) refine_accumulate_kernel(int n, const int* __restrict__ pinv, const T* __restrict__ v,
+                                                               double* __restrict__ x, int add) {
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+    const double d = static_cast<double>(v[pinv != nullptr ? 9 * pinv[k / 9] + k % 9 : k]);
+    x[k] = add ? x[k] + d : d;
+  }
+}
+
+// The lower triangle of the assembled A [n][n] (column-major), rounded to float for a single-precision potrf
+// (CUDADenseCholeskyMixedPrecision::Factorize, dense_cholesky.cc:562-578).  The upper triangle of Af is not written.
+__global__ void __launch_bounds__(256) dense_round_lower_kernel(int n, const double* __restrict__ A, float* __restrict__ Af) {
+  const size_t total = static_cast<size_t>(n) * n;
+  for (size_t e = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; e < total; e += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t j = e / n, i = e - j * n;
+    if (i >= j) Af[e] = static_cast<float>(A[e]);
+  }
+}
+
 }  // namespace b200

@@ -57,10 +57,12 @@ enum KernelId {
   K_SCHUR_PCG,
   K_SPARSE_SCATTER,
   K_SPARSE_FACTOR,
+  K_SPARSE_SOLVE,
   K_DOGLEG_GRAM,
   K_DOGLEG_DIAG,
   K_DOGLEG_GN,
   K_DOGLEG_STEP,
+  K_REFINE,
   K_MISC,
   K_COUNT
 };
@@ -68,7 +70,8 @@ const char* const kKernelNames[K_COUNT] = {"evaluate_jacobian", "evaluate_cost",
                                            "jacobian_multiply", "jacobian_t_multiply", "jtj_multiply", "schur_init",
                                            "schur_multiply", "schur_multiply_big_points", "camera_reduce", "schur_diag_blocks", "invert_9x9", "back_substitute",
                                            "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg",
-                                           "sparse_scatter", "sparse_factor", "dogleg_gram", "dogleg_diagonal", "dogleg_gn", "dogleg_step", "misc"};
+                                           "sparse_scatter", "sparse_factor", "sparse_solve", "dogleg_gram", "dogleg_diagonal", "dogleg_gn", "dogleg_step",
+                                           "refine_convert", "misc"};
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.

@@ -1,6 +1,10 @@
 // SPARSE_SCHUR on the device (SparseSchurComplementSolver, schur_complement_solver.cc:205-335): S + D_f^2, assembled by
 // xs_assemble_kernel, is scattered into the supernodal panels of sparse_plan.cuh and factored by a supernodal Cholesky; the
-// factorisation and both triangular solves run as one persistent kernel.  FP64 throughout.
+// factorisation and both triangular solves run as one persistent kernel.  The factor and the vector it solves in are of one
+// type T: double, or float for use_mixed_precision_solves (solver.h:572-590), where S + D_f^2 is formed in FP64 and rounded
+// once as it is scattered (FloatSuiteSparseCholesky::Factorize, suitesparse.cc:487-498).  Either way the schedule, the tickets
+// and the summation order are the same.  A solve-only launch (kFactor = false) reuses a factor for the corrections of
+// iterative refinement: its forward task runs step 3 alone, which depends on exactly the descendants step 1 does.
 //
 // Tasks: 2 ns tickets, taken in order from a global counter by whichever CTA is free.  Ticket s < ns is the forward task of
 // supernode s: it waits until every descendant that updates s is done, then (left-looking) subtracts their updates from its
@@ -23,6 +27,7 @@ constexpr int kSpMaxCols = 144;   // 9 x kSnMaxCams (sparse_plan.cuh): the wides
 constexpr int kSpTileRows = 64;   // rows of an update tile: two per lane
 constexpr int kSpK = 16;          // columns of the descendant staged per step
 
+template <typename T>
 struct SparseView {
   int C, ns;
   const int* pinv;            // [C] camera -> position
@@ -36,16 +41,17 @@ struct SparseView {
   const int* ntf;             // supernodes each supernode updates
   const long long* blk_off;   // per block of S: offset of its place in L
   const int* blk_ld;          // ... leading dimension there, negative: the block goes in transposed
-  double* L;
-  double* v;                  // [9C] by position: rhs, then y, then x
+  T* L;
+  T* v;                       // [9C] by position: rhs, then y, then x
   int* cnt;                   // [2 ns] dependency counters of the forward / backward tasks
   int* ticket;
   int* fail;                  // set on a non-positive or non-finite pivot
 };
 
 // L <- the blocks of S (as assembled: the upper triangle, without D_f^2) + D_f^2 on the diagonal, into zeroed storage; v <- the
-// reduced right-hand side in the elimination order.  One warp per block of S.
-__global__ void __launch_bounds__(256) sparse_scatter_kernel(SparseView sv, XsView xv, const double* __restrict__ Df,
+// reduced right-hand side in the elimination order, each value rounded to T once.  One warp per block of S.
+template <typename T>
+__global__ void __launch_bounds__(256) sparse_scatter_kernel(SparseView<T> sv, XsView xv, const double* __restrict__ Df,
                                                             const double* __restrict__ rhs) {
   const int lane = threadIdx.x & 31;
   const int nw = gridDim.x * (blockDim.x / 32);
@@ -58,24 +64,30 @@ __global__ void __launch_bounds__(256) sparse_scatter_kernel(SparseView sv, XsVi
       const int u = e / 9, w = e - 9 * u;
       double s = xv.S[81 * static_cast<size_t>(b) + e];
       if (diag && u == w && Df != nullptr) s += Df[9 * i + u] * Df[9 * i + u];
-      sv.L[off + (ldt < 0 ? w + static_cast<long long>(u) * ld : u + static_cast<long long>(w) * ld)] = s;
+      sv.L[off + (ldt < 0 ? w + static_cast<long long>(u) * ld : u + static_cast<long long>(w) * ld)] = static_cast<T>(s);
     }
   }
   for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < 9 * sv.C; k += gridDim.x * blockDim.x)
-    sv.v[9 * sv.pinv[k / 9] + k % 9] = rhs[k];
+    sv.v[9 * sv.pinv[k / 9] + k % 9] = static_cast<T>(rhs[k]);
 }
 
-// sol [9C] in the caller's camera order <- x by position.
-__global__ void __launch_bounds__(256) sparse_gather_kernel(SparseView sv, double* __restrict__ sol) {
+// sol [9C] in the caller's camera order <- x by position, widened to double.
+template <typename T>
+__global__ void __launch_bounds__(256) sparse_gather_kernel(SparseView<T> sv, double* __restrict__ sol) {
   for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < 9 * sv.C; k += gridDim.x * blockDim.x)
-    sol[k] = sv.v[9 * sv.pinv[k / 9] + k % 9];
+    sol[k] = static_cast<double>(sv.v[9 * sv.pinv[k / 9] + k % 9]);
 }
 
 // Dynamic shared memory of sparse_factor_kernel for supernodes of at most W scalar columns: the update stages, the block
 // column being factored [W][9], and y_s / z_s [W].
+template <typename T>
 inline size_t sparse_smem_bytes(int W) {
-  return sizeof(double) * (kSpK * (kSpMaxCols + kSpTileRows) + 9 * static_cast<size_t>(W) + W);
+  return sizeof(T) * (kSpK * (kSpMaxCols + kSpTileRows) + 9 * static_cast<size_t>(W) + W);
 }
+
+template <typename T> struct SpPair;
+template <> struct SpPair<double> { using type = double2; };
+template <> struct SpPair<float> { using type = float2; };
 
 __device__ __forceinline__ void sp_wait(int* c) {
   if (threadIdx.x == 0) {
@@ -90,55 +102,57 @@ __device__ __forceinline__ void sp_release_begin() {
   __syncthreads();
 }
 
-// The forward task of supernode s.
-__device__ void sp_forward(const SparseView& sv, int s, double* sm) {
+// The forward task of supernode s: steps 1 and 2 only when kFactor.
+template <typename T, bool kFactor>
+__device__ void sp_forward(const SparseView<T>& sv, int s, T* sm) {
   const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
   const int f = sv.sn_first[s], w = sv.sn_first[s + 1] - f, W = 9 * w;
   const int rp = sv.row_ptr[s], R = sv.row_ptr[s + 1] - rp, ld = 9 * R;
-  double* Ls = sv.L + sv.val[s];
-  double* sB = sm;                                   // update stages: B [kSpK][kSpMaxCols], then A [kSpK][kSpTileRows]
-  double* sX = sm + kSpK * (kSpMaxCols + kSpTileRows);   // block column K of the rows of the diagonal block: [9w][9]
-  double* sY = sX + 9 * W;                           // y_s
-  __shared__ double sK[81];                          // diagonal block K, column-major
+  T* Ls = sv.L + sv.val[s];
+  T* sB = sm;                                        // update stages: B [kSpK][kSpMaxCols], then A [kSpK][kSpTileRows]
+  T* sX = sm + kSpK * (kSpMaxCols + kSpTileRows);    // block column K of the rows of the diagonal block: [9w][9]
+  T* sY = sX + 9 * W;                                // y_s
+  __shared__ T sK[81];                               // diagonal block K, column-major
   const int u0 = sv.upd_ptr[s], u1 = sv.upd_ptr[s + 1];
+  if (kFactor) {
   // 1. left-looking updates: Ls -= L_d[rows k0.., :] L_d[rows k0..k1-1, :]', in tiles of kSpTileRows rows: A = the tile's
   //    rows and B = the rows in s's columns, both staged kSpK columns of L_d at a time.  Lane l of warp g accumulates rows
   //    2l, 2l + 1 of the tile against column blocks g and g + 8 (9 columns each): 36 products per 2 + 18 shared loads.
-  double* sA = sB + kSpK * kSpMaxCols;
+  T* sA = sB + kSpK * kSpMaxCols;
   for (int q = u0; q < u1; ++q) {
     const int4 u = sv.upd[q];
     const int d = u.x, k0 = u.y, k1 = u.z;
     const int fd = sv.sn_first[d], Wd = 9 * (sv.sn_first[d + 1] - fd);
     const int rpd = sv.row_ptr[d], Rd = sv.row_ptr[d + 1] - rpd, ldd = 9 * Rd;
-    const double* Ld = sv.L + sv.val[d];
+    const T* Ld = sv.L + sv.val[d];
     const int ncb = k1 - k0, nc = 9 * ncb, iend = 9 * Rd;
     for (int r0 = 9 * k0; r0 < iend; r0 += kSpTileRows) {
-      double acc[2][2][9];
+      T acc[2][2][9];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int m = 0; m < 9; ++m) acc[h][0][m] = acc[h][1][m] = 0.0;
+        for (int m = 0; m < 9; ++m) acc[h][0][m] = acc[h][1][m] = T(0);
       for (int t0 = 0; t0 < Wd; t0 += kSpK) {
         __syncthreads();
         for (int e = tid; e < kSpK * kSpTileRows; e += nt) {
           const int k = e / kSpTileRows, r = e - k * kSpTileRows;
-          sA[e] = r0 + r < iend && t0 + k < Wd ? __ldcg(Ld + r0 + r + static_cast<long long>(t0 + k) * ldd) : 0.0;
+          sA[e] = r0 + r < iend && t0 + k < Wd ? __ldcg(Ld + r0 + r + static_cast<long long>(t0 + k) * ldd) : T(0);
         }
         for (int e = tid; e < kSpK * kSpMaxCols; e += nt) {
           const int k = e / kSpMaxCols, c = e - k * kSpMaxCols;
-          sB[e] = c < nc && t0 + k < Wd ? __ldcg(Ld + 9 * k0 + c + static_cast<long long>(t0 + k) * ldd) : 0.0;
+          sB[e] = c < nc && t0 + k < Wd ? __ldcg(Ld + 9 * k0 + c + static_cast<long long>(t0 + k) * ldd) : T(0);
         }
         __syncthreads();
         if (warp < ncb) {
 #pragma unroll 4
           for (int k = 0; k < kSpK; ++k) {
-            const double2 a = *reinterpret_cast<const double2*>(sA + k * kSpTileRows + 2 * lane);
+            const typename SpPair<T>::type a = *reinterpret_cast<const typename SpPair<T>::type*>(sA + k * kSpTileRows + 2 * lane);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const double* b = sB + k * kSpMaxCols + 9 * (warp + 8 * h);
+              const T* b = sB + k * kSpMaxCols + 9 * (warp + 8 * h);
 #pragma unroll
               for (int m = 0; m < 9; ++m) {
-                const double bm = b[m];
+                const T bm = b[m];
                 acc[h][0][m] += a.x * bm;
                 acc[h][1][m] += a.y * bm;
               }
@@ -186,13 +200,13 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
     if (tid == 0) {
       bool bad = false;
       for (int c = 0; c < 9; ++c) {
-        double dcc = sK[c * 9 + c];
+        T dcc = sK[c * 9 + c];
         for (int t = 0; t < c; ++t) dcc -= sK[t * 9 + c] * sK[t * 9 + c];
-        if (!(dcc > 0.0) || !isfinite(dcc)) bad = true;
-        const double lcc = sqrt(dcc);
+        if (!(dcc > T(0)) || !isfinite(dcc)) bad = true;
+        const T lcc = sqrt(dcc);
         sK[c * 9 + c] = lcc;
         for (int r = c + 1; r < 9; ++r) {
-          double a = sK[c * 9 + r];
+          T a = sK[c * 9 + r];
           for (int t = 0; t < c; ++t) a -= sK[t * 9 + r] * sK[t * 9 + c];
           sK[c * 9 + r] = a / lcc;
         }
@@ -202,10 +216,10 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
     __syncthreads();
     if (tid < 81 && tid % 9 >= tid / 9) Ls[9 * K + tid % 9 + static_cast<long long>(9 * K + tid / 9) * ld] = sK[tid];
     const int i0 = 9 * (K + 1);
-    auto solve_row = [&](int i, double* x) {   // x = A_iK L_KK^-T
+    auto solve_row = [&](int i, T* x) {   // x = A_iK L_KK^-T
 #pragma unroll
       for (int c = 0; c < 9; ++c) {
-        double a = Ls[i + static_cast<long long>(9 * K + c) * ld];
+        T a = Ls[i + static_cast<long long>(9 * K + c) * ld];
 #pragma unroll
         for (int t = 0; t < c; ++t) a -= x[t] * sK[t * 9 + c];
         x[c] = a / sK[c * 9 + c];
@@ -214,14 +228,14 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
       for (int c = 0; c < 9; ++c) Ls[i + static_cast<long long>(9 * K + c) * ld] = x[c];
     };
     for (int i = i0 + tid; i < W; i += nt) {   // rows of the diagonal block: staged for the trailing update
-      double x[9];
+      T x[9];
       solve_row(i, x);
 #pragma unroll
       for (int c = 0; c < 9; ++c) sX[(i - i0) * 9 + c] = x[c];
     }
     __syncthreads();
     for (int i = i0 + tid; i < 9 * R; i += nt) {
-      double x[9];
+      T x[9];
       if (i < W) {
 #pragma unroll
         for (int c = 0; c < 9; ++c) x[c] = sX[(i - i0) * 9 + c];
@@ -230,14 +244,15 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
       }
       const int jmax = i < W ? i : W - 1;   // lower triangle of the diagonal block, every column below it
       for (int j = i0; j <= jmax; ++j) {
-        const double* xj = sX + (j - i0) * 9;
-        double a = 0.0;
+        const T* xj = sX + (j - i0) * 9;
+        T a = T(0);
 #pragma unroll
         for (int c = 0; c < 9; ++c) a += x[c] * xj[c];
         Ls[i + static_cast<long long>(j) * ld] -= a;
       }
     }
   }
+  }   // kFactor
   __syncthreads();
   // 3. y_s = L_ss^-1 (rhs_s - sum over the descendants of L_d[rows in s] y_d)
   for (int c = tid; c < W; c += nt) sY[c] = __ldcg(sv.v + 9LL * f + c);
@@ -247,10 +262,10 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
     const int d = u.x, k0 = u.y, k1 = u.z;
     const int fd = sv.sn_first[d], Wd = 9 * (sv.sn_first[d + 1] - fd);
     const int rpd = sv.row_ptr[d], ldd = 9 * (sv.row_ptr[d + 1] - rpd);
-    const double* Ld = sv.L + sv.val[d];
+    const T* Ld = sv.L + sv.val[d];
     const int nc = 9 * (k1 - k0);
     for (int c = tid; c < nc; c += nt) {
-      double a = 0.0;
+      T a = T(0);
       for (int t = 0; t < Wd; ++t) a += __ldcg(Ld + 9 * k0 + c + static_cast<long long>(t) * ldd) * __ldcg(sv.v + 9LL * fd + t);
       sY[9 * (sv.rows[rpd + k0 + c / 9] - f) + c % 9] -= a;
     }
@@ -258,7 +273,7 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
   }
   if (warp == 0) {
     for (int j = 0; j < W; ++j) {
-      const double yj = sY[j] / Ls[j + static_cast<long long>(j) * ld];
+      const T yj = sY[j] / Ls[j + static_cast<long long>(j) * ld];
       __syncwarp();
       if (lane == 0) sY[j] = yj;
       for (int i = j + 1 + lane; i < W; i += 32) sY[i] -= Ls[i + static_cast<long long>(j) * ld] * yj;
@@ -270,15 +285,16 @@ __device__ void sp_forward(const SparseView& sv, int s, double* sm) {
 }
 
 // The backward task of supernode s.
-__device__ void sp_backward(const SparseView& sv, int s, double* sm) {
+template <typename T>
+__device__ void sp_backward(const SparseView<T>& sv, int s, T* sm) {
   const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
   const int f = sv.sn_first[s], w = sv.sn_first[s + 1] - f, W = 9 * w;
   const int rp = sv.row_ptr[s], R = sv.row_ptr[s + 1] - rp, ld = 9 * R;
-  const double* Ls = sv.L + sv.val[s];
-  double* sZ = sm;
+  const T* Ls = sv.L + sv.val[s];
+  T* sZ = sm;
   // z_c = y_c - sum over the rows below of L[i][c] x_i: one warp per column, a fixed butterfly
   for (int c = warp; c < W; c += nt / 32) {
-    double a = 0.0;
+    T a = T(0);
     for (int i = W + lane; i < 9 * R; i += 32) a += Ls[i + static_cast<long long>(c) * ld] * __ldcg(sv.v + 9LL * sv.rows[rp + i / 9] + i % 9);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
@@ -287,7 +303,7 @@ __device__ void sp_backward(const SparseView& sv, int s, double* sm) {
   __syncthreads();
   if (warp == 0) {
     for (int j = W - 1; j >= 0; --j) {
-      const double xj = sZ[j] / Ls[j + static_cast<long long>(j) * ld];
+      const T xj = sZ[j] / Ls[j + static_cast<long long>(j) * ld];
       __syncwarp();
       if (lane == 0) sZ[j] = xj;
       for (int i = lane; i < j; i += 32) sZ[i] -= Ls[j + static_cast<long long>(i) * ld] * xj;
@@ -298,9 +314,12 @@ __device__ void sp_backward(const SparseView& sv, int s, double* sm) {
   for (int c = tid; c < W; c += nt) sv.v[9LL * f + c] = sZ[c];
 }
 
-// The factorisation and both triangular solves: a cooperative launch of at most the resident CTAs, counters reset before it.
-__global__ void __launch_bounds__(kSpThreads, 1) sparse_factor_kernel(SparseView sv) {
-  extern __shared__ double sp_smem[];
+// The factorisation (kFactor) and both triangular solves: a cooperative launch of at most the resident CTAs, counters and
+// ticket reset before it.
+template <typename T, bool kFactor>
+__global__ void __launch_bounds__(kSpThreads, 1) sparse_factor_kernel(SparseView<T> sv) {
+  extern __shared__ __align__(16) unsigned char sp_smem_raw[];
+  T* sp_smem = reinterpret_cast<T*>(sp_smem_raw);
   __shared__ int s_task;
   const int ns = sv.ns;
   for (;;) {
@@ -311,7 +330,7 @@ __global__ void __launch_bounds__(kSpThreads, 1) sparse_factor_kernel(SparseView
     if (t >= 2 * ns) return;
     if (t < ns) {
       sp_wait(sv.cnt + t);
-      sp_forward(sv, t, sp_smem);
+      sp_forward<T, kFactor>(sv, t, sp_smem);
       sp_release_begin();
       if (threadIdx.x == 0) {
         const int n0 = sv.ntf_ptr[t], n1 = sv.ntf_ptr[t + 1];
@@ -321,7 +340,7 @@ __global__ void __launch_bounds__(kSpThreads, 1) sparse_factor_kernel(SparseView
     } else {
       const int s = 2 * ns - 1 - t;
       sp_wait(sv.cnt + ns + s);
-      sp_backward(sv, s, sp_smem);
+      sp_backward<T>(sv, s, sp_smem);
       sp_release_begin();
       if (threadIdx.x == 0)
         for (int k = sv.upd_ptr[s]; k < sv.upd_ptr[s + 1]; ++k) atomicSub(sv.cnt + ns + sv.upd[k].x, 1);

@@ -192,6 +192,19 @@ int b200_dense_schur_solve(b200_handle* h, const double* b, const double* D, dou
  * suitesparse.cc:311-313); single GPU, factor storage up to 48 GB (B200_ERR_UNSUPPORTED otherwise); b == NULL as above. */
 int b200_sparse_schur_solve(b200_handle* h, const double* b, const double* D, double* x, b200_solver_summary* summary);
 
+/* LinearSolver::Options::use_mixed_precision_solves and max_num_refinement_iterations (linear_solver.h:226-227;
+ * Solver::Options, solver.h:572-590) for the following b200_dense_schur_solve / b200_sparse_schur_solve calls on h (both 0
+ * when h is created).  Mixed precision: S + D_f^2 is formed in FP64, rounded to float and factored in float; each solve
+ * rounds its right-hand side to float and widens its result.  Refinement (with or without mixed precision): x_f =
+ * solve(rhs_S), then k times x_f += solve(rhs_S - (S + D_f^2) x_f) with the residual in FP64, 1 + k solves per
+ * factorisation as RefinedSparseCholesky / RefinedDenseCholesky do; the points follow by back substitution of the refined
+ * x_f.  (Ceres' CUDA dense path with mixed precision refines 2k times; the EIGEN / LAPACK and sparse count is followed.)
+ * Summary and failure as above: a non-positive pivot of the (float) factorisation is FAILURE without writing x; failures
+ * of the refinement's solves are ignored.  A flag other than 0 / 1 or k < 0: B200_ERR_INVALID_ARGUMENT.  Mixed-precision
+ * DENSE_SCHUR needs cusolverDnSpotrf / Spotrs in the loaded cuSOLVER (B200_ERR_UNSUPPORTED otherwise); the dense cap
+ * counts the float copy, the sparse one counts the factor in the precision in use. */
+int b200_set_exact_solve_options(b200_handle* h, int use_mixed_precision_solves, int max_num_refinement_iterations);
+
 /* Finer-grained pieces of the same solve, for parity tests (each mirrors one reference class):
  *   ImplicitSchurComplement::Init / rhs / RightMultiplyAndAccumulate / BackSubstitute
  *     (implicit_schur_complement.cc:49-97, :251-276, :106-144, :208-243)
@@ -210,7 +223,11 @@ int b200_block_jacobi_update(b200_handle* h, double* inverse);                  
  * State, residuals, Jacobian, D and the step never leave HBM; only scalars cross the bus.
  * DOGLEG needs an exact solve (solver.cc:431-438): B200_DENSE_SCHUR or B200_SPARSE_SCHUR; with B200_ITERATIVE_SCHUR, or
  * an out-of-range strategy or dogleg type, b200_lm_solve returns B200_ERR_INVALID_ARGUMENT.  A rejected dogleg step
- * keeps its Gauss-Newton step and gradient and costs no solve; its record has linear_solver_iterations 0. */
+ * keeps its Gauss-Newton step and gradient and costs no solve; its record has linear_solver_iterations 0.
+ * use_mixed_precision_solves / max_num_refinement_iterations apply to the call's exact solves, the Gauss-Newton solves of
+ * DOGLEG included, as b200_set_exact_solve_options would; the handle's own values are restored when the call returns, also
+ * on an error.  Mixed precision with B200_ITERATIVE_SCHUR is B200_ERR_INVALID_ARGUMENT (solver.cc:298-300); k is ignored
+ * there. */
 typedef struct b200_lm_options { /* Solver::Options subset, include/ceres/solver.h:232-632 */
   int32_t max_num_iterations;              /* bundle_adjuster.cc:121 (5) */
   int32_t jacobi_scaling;                  /* 1 */
@@ -226,6 +243,8 @@ typedef struct b200_lm_options { /* Solver::Options subset, include/ceres/solver
   b200_solver_options linear_solver;
   int32_t trust_region_strategy_type;      /* B200_LEVENBERG_MARQUARDT (default) or B200_DOGLEG */
   int32_t dogleg_type;                     /* B200_TRADITIONAL_DOGLEG (default) or B200_SUBSPACE_DOGLEG */
+  int32_t use_mixed_precision_solves;      /* solver.h:572-580 (0) */
+  int32_t max_num_refinement_iterations;   /* :582-590 (0) */
 } b200_lm_options;
 typedef struct b200_lm_iteration { /* IterationSummary, include/ceres/iteration_callback.h */
   int32_t iteration, linear_solver_iterations, step_is_valid, step_is_successful;

@@ -5,8 +5,14 @@ trust-region strategy (LM, traditional and subspace DOGLEG): iterations per seco
 after K iterations and the rejected steps; the symbolic statistics and the host analysis time, and the card's name and power
 limit.
 
+With --precision, the precision / refinement axis of the exact solves instead (b200_set_exact_solve_options and the matching
+b200_lm_options fields): FP64, FP64 with 2 refinements, and mixed precision (float factorisation) with k = 0, 1 and 3, each with
+SPARSE_SCHUR: the factor kernel's time and the solve's, its termination, b200_lm_solve's iterations per second over
+--lm-iterations LM iterations, its factorisation FAILUREs (invalid steps) and rejected steps, and the cost reached relative
+to FP64's.
+
     python tools/bench_exact_schur.py [--reps 5] [--lm-iterations 5] [--problems ladybug-1723,...]
-                                      [--strategies lm,traditional_dogleg,subspace_dogleg] [--out results.json]
+                                      [--strategies lm,traditional_dogleg,subspace_dogleg] [--precision] [--out results.json]
 
 One JSON line per problem on stdout.  Needs an H100; nothing is written unless --out is given.
 """
@@ -79,12 +85,44 @@ def lm_rate(gpu, state, solver_type, iterations, strategy=cs.LEVENBERG_MARQUARDT
                 invalid=sum(1 for r in recs[1:] if not r["step_is_valid"]))
 
 
+# precision / refinement axis: (name, use_mixed_precision_solves, max_num_refinement_iterations)
+PRECISIONS = [("fp64", 0, 0), ("fp64_k2", 0, 2), ("mixed_k0", 1, 0), ("mixed_k1", 1, 1), ("mixed_k3", 1, 3)]
+
+
+def precision_axis(gpu, state, res, D, reps, iterations):
+    out = {}
+    for name, mixed, k in PRECISIONS:   # every solve before any LM run: b200_lm_solve leaves its own Jacobian on the handle
+        gpu.set_exact_solve_options(mixed, k)
+        x, term, ms, kernels = timed_solves(gpu, gpu.sparse_schur_solve, res, D, reps)
+        out[name] = dict(solve_ms=round(ms, 3), factor_ms=kernels.get("sparse_factor"), solve_only_ms=kernels.get("sparse_solve"),
+                         termination=int(term), x=x)
+    gpu.set_exact_solve_options(0, 0)
+    for name, mixed, k in PRECISIONS:
+        kw = dict(linear_solver_type=cs.SPARSE_SCHUR, use_mixed_precision_solves=mixed, max_num_refinement_iterations=k)
+        gpu.lm_solve(state, gpu.lm_options(max_num_iterations=1, **kw))   # warm-up
+        gpu.synchronize()
+        t = time.perf_counter()
+        _, recs = gpu.lm_solve(state, gpu.lm_options(max_num_iterations=iterations, **kw))
+        dt = time.perf_counter() - t
+        its = len(recs) - 1
+        out[name].update(lm_its_per_s=its / dt, lm_iterations=its, lm_cost=recs[-1]["cost"],
+                         lm_failures=sum(1 for r in recs[1:] if not r["step_is_valid"]),
+                         lm_rejected=sum(1 for r in recs[1:] if r["step_is_valid"] and not r["step_is_successful"]))
+    x64 = out["fp64"]["x"]
+    for v in out.values():
+        x = v.pop("x")
+        v["relerr_vs_fp64"] = float(np.linalg.norm(x - x64) / np.linalg.norm(x64))
+        v["lm_cost_vs_fp64"] = v["lm_cost"] / out["fp64"]["lm_cost"] - 1.0
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--lm-iterations", type=int, default=5)
     ap.add_argument("--problems", default=",".join(PROBLEMS))
     ap.add_argument("--strategies", default=",".join(n for n, _, _ in STRATEGIES))
+    ap.add_argument("--precision", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     device = card()
@@ -103,6 +141,12 @@ def main():
         gpu.scale_columns(s)
         D = np.sqrt(np.clip(gpu.squared_column_norm(), 1e-6, 1e32) / 1e4)
         row = dict(problem=name, device=device, C=rp.C, P=rp.P, N=rp.N, analysis_ms=round(analysis_ms, 2), **st)
+        if a.precision:
+            row["precision"] = precision_axis(gpu, state, res, D, a.reps, a.lm_iterations)
+            gpu.close()
+            print(json.dumps(row), flush=True)
+            results.append(row)
+            continue
         xs, ts, row["sparse_ms"], row["sparse_kernels_ms"] = timed_solves(gpu, gpu.sparse_schur_solve, res, D, a.reps)
         xd, td, row["dense_ms"], row["dense_kernels_ms"] = timed_solves(gpu, gpu.dense_schur_solve, res, D, a.reps)
         row["terminations"] = [int(ts), int(td)]
