@@ -5,5 +5,5 @@ or without a GPU raises."""
 from . import bal  # noqa: F401
 from .binding import (B200Error, Problem, lib, nccl_unique_id, plan_point_order, plan_sparse_schur, LIB_PATH, SYMBOLS,  # noqa: F401
                       PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION, ITERATIVE_SCHUR, DENSE_SCHUR,
-                      SPARSE_SCHUR, SPARSE_STATS, LEVENBERG_MARQUARDT, DOGLEG, TRADITIONAL_DOGLEG, SUBSPACE_DOGLEG, LOSS_TRIVIAL, LOSS_HUBER,
+                      SPARSE_SCHUR, SPARSE_STATS, LEVENBERG_MARQUARDT, DOGLEG, TRADITIONAL_DOGLEG, SUBSPACE_DOGLEG, AMD, NESDIS, LOSS_TRIVIAL, LOSS_HUBER,
                       LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR)

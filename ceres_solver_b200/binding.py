@@ -25,9 +25,11 @@ PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERI
 ITERATIVE_SCHUR, DENSE_SCHUR, SPARSE_SCHUR = 0, 1, 2
 LEVENBERG_MARQUARDT, DOGLEG = 0, 1                  # trust_region_strategy_type
 TRADITIONAL_DOGLEG, SUBSPACE_DOGLEG = 0, 1          # dogleg_type
+AMD, NESDIS = 0, 1                                  # linear_solver_ordering_type
 # b200_plan_sparse_schur's statistics (B200_SPARSE_STAT_*), in order
 SPARSE_STATS = ("s_blocks", "l_blocks", "l_blocks_caller", "l_blocks_min_degree", "flops_caller", "flops_min_degree",
-                "supernodes", "tree_height", "order", "factor_bytes")
+                "supernodes", "tree_height", "order", "factor_bytes", "flops", "critical_path_supernodes",
+                "critical_path_flops")
 LOSS_TRIVIAL, LOSS_HUBER = 0, 1
 
 
@@ -64,7 +66,8 @@ class LmOptions(C.Structure):
                 ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
                 ("linear_solver", SolverOptions), ("trust_region_strategy_type", C.c_int32), ("dogleg_type", C.c_int32),
-                ("use_mixed_precision_solves", C.c_int32), ("max_num_refinement_iterations", C.c_int32)]
+                ("use_mixed_precision_solves", C.c_int32), ("max_num_refinement_iterations", C.c_int32),
+                ("linear_solver_ordering_type", C.c_int32)]
 
 
 class LmIteration(C.Structure):
@@ -82,11 +85,12 @@ class KernelStat(C.Structure):
 
 # Every symbol include/b200ba.h declares (tests/test_abi.py checks the library exports all of them).
 SYMBOLS = [
-    "b200_plan_point_order", "b200_plan_sparse_schur", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
+    "b200_plan_point_order", "b200_plan_sparse_schur", "b200_plan_sparse_schur_ordered", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
     "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
-    "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options", "b200_schur_init", "b200_schur_rhs", "b200_schur_ete_inverse", "b200_schur_multiply",
+    "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options",
+    "b200_set_linear_solver_ordering_type", "b200_schur_init", "b200_schur_rhs", "b200_schur_ete_inverse", "b200_schur_multiply",
     "b200_schur_back_substitute", "b200_schur_jacobi_update", "b200_block_jacobi_update",
     "b200_lm_options_default", "b200_lm_solve", "b200_profile_enable", "b200_stats_reset", "b200_stats_get",
     "b200_total_launches", "b200_synchronize", "b200_transfer_bytes",
@@ -137,9 +141,9 @@ def plan_point_order(num_cameras, num_points, cam_idx, pt_idx, num_chunks=132):
     return perm, [int(m) for m in metrics], choice.value
 
 
-def plan_sparse_schur(num_cameras, num_points, cam_idx, pt_idx):
-    """Host-only: the symbolic analysis b200_sparse_schur_solve runs for this structure.  Returns (camera elimination order,
-    dict of SPARSE_STATS)."""
+def plan_sparse_schur(num_cameras, num_points, cam_idx, pt_idx, ordering_type=AMD):
+    """Host-only: the symbolic analysis b200_sparse_schur_solve runs for this structure under `ordering_type` (AMD or
+    NESDIS).  Returns (camera elimination order, dict of SPARSE_STATS)."""
     cam = np.ascontiguousarray(cam_idx, dtype=np.int32)
     pt = np.ascontiguousarray(pt_idx, dtype=np.int32)
     d = BaDesc()
@@ -148,7 +152,7 @@ def plan_sparse_schur(num_cameras, num_points, cam_idx, pt_idx):
     d.pt_idx = pt.ctypes.data_as(_ip)
     perm = np.zeros(int(num_cameras), dtype=np.int32)
     stats = (C.c_int64 * len(SPARSE_STATS))()
-    _check(lib().b200_plan_sparse_schur(C.byref(d), perm.ctypes.data_as(_ip), stats))
+    _check(lib().b200_plan_sparse_schur_ordered(C.byref(d), int(ordering_type), perm.ctypes.data_as(_ip), stats))
     return perm, {k: int(v) for k, v in zip(SPARSE_STATS, stats)}
 
 
@@ -292,6 +296,11 @@ class Problem:
         """LinearSolver::Options::use_mixed_precision_solves / max_num_refinement_iterations of the later dense and sparse
         Schur solves on this handle."""
         _check(lib().b200_set_exact_solve_options(self.h, int(use_mixed_precision_solves), int(max_num_refinement_iterations)))
+
+    def set_linear_solver_ordering_type(self, ordering_type):
+        """Solver::Options::linear_solver_ordering_type (AMD or NESDIS) of the later sparse Schur solves on this handle; a
+        change drops the handle's sparse analysis, which the next sparse solve runs again."""
+        _check(lib().b200_set_linear_solver_ordering_type(self.h, int(ordering_type)))
 
     def model_cost_change(self, step):
         out = C.c_double(0.0)

@@ -304,6 +304,7 @@ struct b200_handle {
   // (linear_solver.h:226-227) of the DENSE_SCHUR and SPARSE_SCHUR solves
   bool mixed = false;
   int refine = 0;
+  int ordering = B200_AMD;    // b200_set_linear_solver_ordering_type: the camera order of the SPARSE_SCHUR analysis
   HostMirrors hm;             // host-boundary LM loop vectors
   // launch geometry
   int grid_tile[K_COUNT];
@@ -327,6 +328,15 @@ int dev_alloc(b200_handle* h, T** p, size_t n) {
   CU(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
   h->allocs.push_back(*p);
   return B200_OK;
+}
+// Frees one allocation of dev_alloc before the handle is destroyed.
+template <typename T>
+void dev_free(b200_handle* h, T*& p) {
+  if (p == nullptr) return;
+  void* q = const_cast<void*>(static_cast<const void*>(p));
+  h->allocs.erase(std::find(h->allocs.begin(), h->allocs.end(), q));
+  cudaFree(q);
+  p = nullptr;
 }
 // dev_alloc of a device copy of `src`, uploaded on the handle's stream.
 template <typename T>
@@ -1123,7 +1133,7 @@ int sparse_analyse(b200_handle* h) {
   XsPattern xp;
   xs_pattern(h->C, h->N, h->h_cam_idx.data(), h->h_pt_idx.data(), h->h_pt_ptr.data(), &xp);
   SparsePlan sp;
-  plan_sparse_schur(h->C, xp.blk_row, xp.blk_col, &sp);
+  plan_sparse_schur(h->C, xp.blk_row, xp.blk_col, h->ordering, &sp);
   // the cap counts the bytes of the precision in use (sparse_factor_solve); none fits when even a float factor does not
   if (4.0 * static_cast<double>(sp.storage) > kFactorMaxBytes)
     return fail(B200_ERR_UNSUPPORTED, "sparse factor of %d cameras needs %.1f GB", h->C, 4.0 * static_cast<double>(sp.storage) / 1e9);
@@ -1154,6 +1164,7 @@ int sparse_analyse(b200_handle* h) {
   OK(upload(h, sp.upd, &v.upd));
   OK(upload(h, sp.ntf_ptr, &v.ntf_ptr));
   OK(upload(h, sp.ntf, &v.ntf));
+  OK(upload(h, sp.order, &v.order));
   OK(upload(h, sp.blk_off, &v.blk_off));
   OK(upload(h, sp.blk_ld, &v.blk_ld));
   OK(upload(h, sp.cnt, &h->d_sp_cnt_init));
@@ -1187,15 +1198,48 @@ int sparse_analyse(b200_handle* h) {
     const int64_t* st = sp.stats;
     fprintf(stderr,
             "[b200ba] sparse S plan: %lld blocks of S, L %lld blocks (caller's order %lld, minimum degree %lld), flops caller %.3g / "
-            "minimum degree %.3g -> %s, %d supernodes (widest %d columns), tree height %lld, factor %.1f MB, %d CTAs\n",
+            "minimum degree %.3g -> %s, %d supernodes (widest %d columns), tree height %lld, factor %.1f MB, %d CTAs, "
+            "critical path %lld supernodes / %.3g flops of %.3g\n",
             static_cast<long long>(st[B200_SPARSE_STAT_S_BLOCKS]), static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS]),
             static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS_CALLER]), static_cast<long long>(st[B200_SPARSE_STAT_L_BLOCKS_MIN_DEGREE]),
             static_cast<double>(st[B200_SPARSE_STAT_FLOPS_CALLER]), static_cast<double>(st[B200_SPARSE_STAT_FLOPS_MIN_DEGREE]),
-            st[B200_SPARSE_STAT_ORDER] ? "minimum degree" : "caller's order", sp.ns, sp.max_width,
-            static_cast<long long>(st[B200_SPARSE_STAT_TREE_HEIGHT]), 8.0 * static_cast<double>(sp.storage) / 1e6, h->sp_grid);
+            st[B200_SPARSE_STAT_ORDER] == 2 ? "nested dissection" : st[B200_SPARSE_STAT_ORDER] ? "minimum degree" : "caller's order",
+            sp.ns, sp.max_width, static_cast<long long>(st[B200_SPARSE_STAT_TREE_HEIGHT]), 8.0 * static_cast<double>(sp.storage) / 1e6,
+            h->sp_grid, static_cast<long long>(st[B200_SPARSE_STAT_CRITICAL_PATH_SUPERNODES]),
+            static_cast<double>(st[B200_SPARSE_STAT_CRITICAL_PATH_FLOPS]), static_cast<double>(st[B200_SPARSE_STAT_FLOPS]));
   }
   h->sp_ready = true;
   return B200_OK;
+}
+
+// Undoes sparse_analyse: the plan's arrays and both factors (the arrays xs_assemble_dev reads stay: they do not depend on
+// the camera order).
+void sparse_drop(b200_handle* h) {
+  if (h->stream != nullptr) cudaStreamSynchronize(h->stream);
+  SparseView<double>& v = h->spv;
+  dev_free(h, v.pinv);
+  dev_free(h, v.sn_first);
+  dev_free(h, v.row_ptr);
+  dev_free(h, v.rows);
+  dev_free(h, v.val);
+  dev_free(h, v.upd_ptr);
+  dev_free(h, v.upd);
+  dev_free(h, v.ntf_ptr);
+  dev_free(h, v.ntf);
+  dev_free(h, v.order);
+  dev_free(h, v.blk_off);
+  dev_free(h, v.blk_ld);
+  dev_free(h, v.L);
+  dev_free(h, v.v);
+  dev_free(h, v.cnt);
+  dev_free(h, v.ticket);
+  dev_free(h, h->spv32.L);
+  dev_free(h, h->spv32.v);
+  dev_free(h, h->d_sp_cnt_init);
+  h->spv = SparseView<double>{};
+  h->spv32 = SparseView<float>{};
+  h->sp_storage = 0;
+  h->sp_ready = false;
 }
 
 // The factorisation of S + D_f^2 in T, its solve and the refinement's (1 + h->refine solves), into h->d_sol; false in *ok
@@ -2139,6 +2183,13 @@ int b200_plan_point_order(const b200_ba_desc* desc, int num_chunks, int32_t* per
 }
 
 int b200_plan_sparse_schur(const b200_ba_desc* desc, int32_t* cam_perm_out, int64_t stats_out[B200_SPARSE_STATS]) {
+  return b200_plan_sparse_schur_ordered(desc, B200_AMD, cam_perm_out, stats_out);
+}
+
+int b200_plan_sparse_schur_ordered(const b200_ba_desc* desc, int ordering_type, int32_t* cam_perm_out,
+                                   int64_t stats_out[B200_SPARSE_STATS]) {
+  if (ordering_type != B200_AMD && ordering_type != B200_NESDIS)
+    return fail(B200_ERR_INVALID_ARGUMENT, "linear_solver_ordering_type must be B200_AMD or B200_NESDIS, not %d", ordering_type);
   if (desc == nullptr || desc->cam_idx == nullptr || desc->pt_idx == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   const int C = desc->num_cameras, P = desc->num_points;
   const int N = static_cast<int>(desc->num_observations);
@@ -2148,7 +2199,7 @@ int b200_plan_sparse_schur(const b200_ba_desc* desc, int32_t* cam_perm_out, int6
   XsPattern xp;   // the block pattern of S does not depend on the point order: the caller's rows give the handle's pattern
   xs_pattern(C, N, desc->cam_idx, desc->pt_idx, ptr.data(), &xp);
   SparsePlan sp;
-  plan_sparse_schur(C, xp.blk_row, xp.blk_col, &sp);
+  plan_sparse_schur(C, xp.blk_row, xp.blk_col, ordering_type, &sp);
   if (cam_perm_out != nullptr)
     for (int k = 0; k < C; ++k) cam_perm_out[k] = sp.perm[k];
   if (stats_out != nullptr)
@@ -2188,6 +2239,7 @@ void b200_lm_options_default(b200_lm_options* o) {
   o->dogleg_type = B200_TRADITIONAL_DOGLEG;
   o->use_mixed_precision_solves = 0;     // solver.h:572-580
   o->max_num_refinement_iterations = 0;  // :582-590
+  o->linear_solver_ordering_type = B200_AMD;   // solver.h:410
 }
 
 int b200_create(const b200_ba_desc* desc, b200_handle** out) {
@@ -2778,6 +2830,17 @@ int b200_set_exact_solve_options(b200_handle* h, int use_mixed_precision_solves,
   return B200_OK;
 }
 
+int b200_set_linear_solver_ordering_type(b200_handle* h, int type) {
+  if (h == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+  if (type != B200_AMD && type != B200_NESDIS)
+    return fail(B200_ERR_INVALID_ARGUMENT, "linear_solver_ordering_type must be B200_AMD or B200_NESDIS, not %d", type);
+  if (type == h->ordering) return B200_OK;
+  CU(cudaSetDevice(h->device));
+  sparse_drop(h);
+  h->ordering = type;
+  return B200_OK;
+}
+
 int b200_schur_init(b200_handle* h, const double* b, const double* D) {
   if (h == nullptr || b == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   CU(cudaSetDevice(h->device));
@@ -2864,14 +2927,19 @@ int b200_lm_solve(b200_handle* h, const b200_lm_options* opt, double* state_inou
   // the exact solves of this call (the host-boundary loop's public calls included) use the call's options; the handle's
   // own are restored on every exit
   const bool mixed0 = h->mixed;
-  const int refine0 = h->refine;
+  const int refine0 = h->refine, ordering0 = h->ordering;
   OK(b200_set_exact_solve_options(h, opt->use_mixed_precision_solves, opt->max_num_refinement_iterations));
   struct Restore {
     b200_handle* h;
     bool mixed;
-    int refine;
-    ~Restore() { h->mixed = mixed; h->refine = refine; }
-  } restore{h, mixed0, refine0};
+    int refine, ordering;
+    ~Restore() {
+      h->mixed = mixed;
+      h->refine = refine;
+      b200_set_linear_solver_ordering_type(h, ordering);
+    }
+  } restore{h, mixed0, refine0, ordering0};
+  OK(b200_set_linear_solver_ordering_type(h, opt->linear_solver_ordering_type));
   CU(cudaSetDevice(h->device));
   *num_records = 0;
   auto run = [&](auto side) {

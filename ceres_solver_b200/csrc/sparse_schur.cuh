@@ -6,11 +6,14 @@
 // and the summation order are the same.  A solve-only launch (kFactor = false) reuses a factor for the corrections of
 // iterative refinement: its forward task runs step 3 alone, which depends on exactly the descendants step 1 does.
 //
-// Tasks: 2 ns tickets, taken in order from a global counter by whichever CTA is free.  Ticket s < ns is the forward task of
-// supernode s: it waits until every descendant that updates s is done, then (left-looking) subtracts their updates from its
-// panel in ascending order of descendant, factors the panel (right-looking, one 9-column block at a time), and computes its
-// part of y = L^-1 rhs.  Ticket 2 ns - 1 - s is the backward task of s: once every supernode holding one of its rows below is
-// done (a root: once its own forward task is), x_s = L_ss^-T (y_s - L_below,s' x_below).  A task only waits on tasks with
+// Tasks: 2 ns tickets, taken in order from a global counter by whichever CTA is free.  Ticket t < ns is the forward task of
+// supernode s = order[t]: it waits until every descendant that updates s is done, then (left-looking) subtracts their updates
+// from its panel in ascending order of descendant, factors the panel (right-looking, one 9-column block at a time), and
+// computes its part of y = L^-1 rhs.  Ticket t >= ns is the backward task of s = order[2 ns - 1 - t]: once every supernode
+// holding one of its rows below is done (a root: once its own forward task is), x_s = L_ss^-T (y_s - L_below,s' x_below).
+// `order` (sparse_plan.cuh) is topological, every descendant before its ancestors: the identity with AMD, leaves first with
+// nested dissection.  So a forward task waits only on descendants, whose forward tickets are smaller; a backward task only on
+// ancestors, whose backward tickets are smaller, or (a root) on its own forward ticket.  A task thus only waits on tasks with
 // smaller tickets, which have all been taken by CTAs that are running (the launch is cooperative: every CTA is resident), so
 // the walk cannot deadlock.  Each panel entry and each entry of y and x is written by the one CTA that owns the supernode, in
 // a fixed order: no atomics on values, and the result is bitwise reproducible.  The counters themselves are atomics.
@@ -39,6 +42,7 @@ struct SparseView {
   const int4* upd;            // {descendant d, k0, k1, 0}
   const int* ntf_ptr;         // [ns + 1]
   const int* ntf;             // supernodes each supernode updates
+  const int* order;           // [ns] supernode of each forward ticket, topological
   const long long* blk_off;   // per block of S: offset of its place in L
   const int* blk_ld;          // ... leading dimension there, negative: the block goes in transposed
   T* L;
@@ -329,16 +333,17 @@ __global__ void __launch_bounds__(kSpThreads, 1) sparse_factor_kernel(SparseView
     const int t = s_task;
     if (t >= 2 * ns) return;
     if (t < ns) {
-      sp_wait(sv.cnt + t);
-      sp_forward<T, kFactor>(sv, t, sp_smem);
+      const int s = sv.order[t];
+      sp_wait(sv.cnt + s);
+      sp_forward<T, kFactor>(sv, s, sp_smem);
       sp_release_begin();
       if (threadIdx.x == 0) {
-        const int n0 = sv.ntf_ptr[t], n1 = sv.ntf_ptr[t + 1];
+        const int n0 = sv.ntf_ptr[s], n1 = sv.ntf_ptr[s + 1];
         for (int k = n0; k < n1; ++k) atomicSub(sv.cnt + sv.ntf[k], 1);
-        if (n0 == n1) atomicSub(sv.cnt + ns + t, 1);   // a root: its backward task may start
+        if (n0 == n1) atomicSub(sv.cnt + ns + s, 1);   // a root: its backward task may start
       }
     } else {
-      const int s = 2 * ns - 1 - t;
+      const int s = sv.order[2 * ns - 1 - t];
       sp_wait(sv.cnt + ns + s);
       sp_backward<T>(sv, s, sp_smem);
       sp_release_begin();

@@ -85,12 +85,18 @@ typedef struct b200_ba_desc {
  * metrics_out = distinct cameras per 1/num_chunks of the rows, summed, for {caller's order, by camera arc, by mean camera,
  * by smallest camera}; *choice_out = which of the four was taken (0 = the caller's order is kept). */
 int b200_plan_point_order(const b200_ba_desc* desc, int num_chunks, int32_t* perm_out, int64_t metrics_out[4], int* choice_out);
+/* LinearSolverOrderingType (include/ceres/types.h:208, same numeric order): how SPARSE_SCHUR orders the reduced camera
+ * system.  B200_AMD: the caller's order or minimum degree, whichever needs fewer flops; B200_NESDIS: nested dissection of the
+ * camera graph (solver.h:410).  DENSE_SCHUR and ITERATIVE_SCHUR ignore it. */
+enum { B200_AMD = 0, B200_NESDIS = 1 };
 /* The symbolic analysis b200_sparse_schur_solve runs at its first call on a handle of this structure.  Host-only, needs no GPU:
  * cam_perm_out[k] = camera eliminated k-th ([C], may be NULL); stats_out (may be NULL), indexed by B200_SPARSE_STAT_*:
  * blocks of the upper triangle of S (diagonal included); blocks of L (diagonal included) in the chosen order, in the caller's
  * order and in the minimum-degree order; factor flops in the caller's and in the minimum-degree order; supernodes; height of
  * the elimination tree (nodes on its longest path); which order was taken (0 the caller's, 1 minimum degree: the one of
- * fewer flops, the caller's on a tie; minimum degree is tried up to 32768 cameras); bytes of factor storage. */
+ * fewer flops, the caller's on a tie; minimum degree is tried up to 32768 cameras and only with B200_AMD, and reported with
+ * the caller's counts where it is not; 2 nested dissection); bytes of factor storage; factor flops in the order taken; and,
+ * over the tree of supernodes, the most supernodes and the most flops on one path from a leaf to a root. */
 enum {
   B200_SPARSE_STAT_S_BLOCKS = 0,
   B200_SPARSE_STAT_L_BLOCKS,
@@ -102,9 +108,16 @@ enum {
   B200_SPARSE_STAT_TREE_HEIGHT,
   B200_SPARSE_STAT_ORDER,
   B200_SPARSE_STAT_FACTOR_BYTES,
+  B200_SPARSE_STAT_FLOPS,
+  B200_SPARSE_STAT_CRITICAL_PATH_SUPERNODES,
+  B200_SPARSE_STAT_CRITICAL_PATH_FLOPS,
   B200_SPARSE_STATS
 };
 int b200_plan_sparse_schur(const b200_ba_desc* desc, int32_t* cam_perm_out, int64_t stats_out[B200_SPARSE_STATS]);
+/* The same analysis under a given ordering type (B200_AMD: b200_plan_sparse_schur; B200_NESDIS); any other value:
+ * B200_ERR_INVALID_ARGUMENT. */
+int b200_plan_sparse_schur_ordered(const b200_ba_desc* desc, int ordering_type, int32_t* cam_perm_out,
+                                   int64_t stats_out[B200_SPARSE_STATS]);
 int b200_nccl_unique_id(void* out128);
 int b200_create(const b200_ba_desc* desc, b200_handle** out);
 void b200_destroy(b200_handle* h);
@@ -205,6 +218,11 @@ int b200_sparse_schur_solve(b200_handle* h, const double* b, const double* D, do
  * counts the float copy, the sparse one counts the factor in the precision in use. */
 int b200_set_exact_solve_options(b200_handle* h, int use_mixed_precision_solves, int max_num_refinement_iterations);
 
+/* Solver::Options::linear_solver_ordering_type (solver.h:410) of the following b200_sparse_schur_solve calls on h (B200_AMD
+ * when h is created).  A different type drops h's sparse analysis and factor storage, so the next sparse solve analyses
+ * again; the same type is a no-op.  A value other than B200_AMD / B200_NESDIS: B200_ERR_INVALID_ARGUMENT. */
+int b200_set_linear_solver_ordering_type(b200_handle* h, int type);
+
 /* Finer-grained pieces of the same solve, for parity tests (each mirrors one reference class):
  *   ImplicitSchurComplement::Init / rhs / RightMultiplyAndAccumulate / BackSubstitute
  *     (implicit_schur_complement.cc:49-97, :251-276, :106-144, :208-243)
@@ -227,7 +245,9 @@ int b200_block_jacobi_update(b200_handle* h, double* inverse);                  
  * use_mixed_precision_solves / max_num_refinement_iterations apply to the call's exact solves, the Gauss-Newton solves of
  * DOGLEG included, as b200_set_exact_solve_options would; the handle's own values are restored when the call returns, also
  * on an error.  Mixed precision with B200_ITERATIVE_SCHUR is B200_ERR_INVALID_ARGUMENT (solver.cc:298-300); k is ignored
- * there. */
+ * there.  linear_solver_ordering_type applies to the call's sparse solves in the same way, as
+ * b200_set_linear_solver_ordering_type would, and the handle's own type is restored on every exit: a call whose type
+ * differs from the handle's analyses once for itself, and the handle's next sparse solve analyses again. */
 typedef struct b200_lm_options { /* Solver::Options subset, include/ceres/solver.h:232-632 */
   int32_t max_num_iterations;              /* bundle_adjuster.cc:121 (5) */
   int32_t jacobi_scaling;                  /* 1 */
@@ -245,6 +265,7 @@ typedef struct b200_lm_options { /* Solver::Options subset, include/ceres/solver
   int32_t dogleg_type;                     /* B200_TRADITIONAL_DOGLEG (default) or B200_SUBSPACE_DOGLEG */
   int32_t use_mixed_precision_solves;      /* solver.h:572-580 (0) */
   int32_t max_num_refinement_iterations;   /* :582-590 (0) */
+  int32_t linear_solver_ordering_type;     /* solver.h:410: B200_AMD (default) or B200_NESDIS */
 } b200_lm_options;
 typedef struct b200_lm_iteration { /* IterationSummary, include/ceres/iteration_callback.h */
   int32_t iteration, linear_solver_iterations, step_is_valid, step_is_successful;

@@ -11,8 +11,14 @@ SPARSE_SCHUR: the factor kernel's time and the solve's, its termination, b200_lm
 --lm-iterations LM iterations, its factorisation FAILUREs (invalid steps) and rejected steps, and the cost reached relative
 to FP64's.
 
+With --ordering amd,nesdis, the linear_solver_ordering_type axis of SPARSE_SCHUR instead (b200_set_linear_solver_ordering_type
+and b200_lm_options.linear_solver_ordering_type), --runs times with the orderings alternating on one handle: the plan's
+statistics and host analysis time, the factor kernel's time and the solve's, LM and traditional DOGLEG iterations per second,
+and |dx| / |x| against the AMD solve; DENSE_SCHUR's LM rate once per problem for comparison.
+
     python tools/bench_exact_schur.py [--reps 5] [--lm-iterations 5] [--problems ladybug-1723,...]
-                                      [--strategies lm,traditional_dogleg,subspace_dogleg] [--precision] [--out results.json]
+                                      [--strategies lm,traditional_dogleg,subspace_dogleg] [--precision]
+                                      [--ordering amd,nesdis [--runs 3]] [--out results.json]
 
 One JSON line per problem on stdout.  Needs an H100; nothing is written unless --out is given.
 """
@@ -67,11 +73,11 @@ STRATEGIES = [("lm", cs.LEVENBERG_MARQUARDT, cs.TRADITIONAL_DOGLEG), ("tradition
               ("subspace_dogleg", cs.DOGLEG, cs.SUBSPACE_DOGLEG)]
 
 
-def lm_rate(gpu, state, solver_type, iterations, strategy=cs.LEVENBERG_MARQUARDT, dogleg_type=cs.TRADITIONAL_DOGLEG):
+def lm_rate(gpu, state, solver_type, iterations, strategy=cs.LEVENBERG_MARQUARDT, dogleg_type=cs.TRADITIONAL_DOGLEG, **extra):
     """b200_lm_solve for `iterations` iterations: iterations per second, the cost reached, factorisations per iteration
     (launches of the dense assembly or of the sparse factor kernel: a rejected DOGLEG step reuses its factorisation, a
     rejected LM step does not) and the rejected and invalid steps of the run."""
-    kw = dict(linear_solver_type=solver_type, trust_region_strategy_type=strategy, dogleg_type=dogleg_type)
+    kw = dict(linear_solver_type=solver_type, trust_region_strategy_type=strategy, dogleg_type=dogleg_type, **extra)
     gpu.lm_solve(state, gpu.lm_options(max_num_iterations=1, **kw))   # warm-up
     gpu.synchronize()
     gpu.stats_reset()
@@ -116,6 +122,49 @@ def precision_axis(gpu, state, res, D, reps, iterations):
     return out
 
 
+ORDERINGS = {"amd": cs.AMD, "nesdis": cs.NESDIS}
+ORDER_STATS = ("flops", "l_blocks", "supernodes", "tree_height", "critical_path_supernodes", "critical_path_flops",
+               "factor_bytes", "order")
+
+
+def ordering_axis(gpu, rp, state, res, D, names, runs, reps, iterations):
+    """Per ordering: the statistics, then per run (orderings alternating) the analysis time, the factor and solve times, the
+    LM and traditional DOGLEG rates with SPARSE_SCHUR and |dx| / |x| against the AMD solve of the same run."""
+    out = {n: dict(runs=[]) for n in names}
+    for n in names:
+        _, st = cs.plan_sparse_schur(rp.C, rp.P, rp.row_cam, rp.row_pt, ORDERINGS[n])
+        out[n].update({k: st[k] for k in ORDER_STATS})
+    for run in range(runs):
+        xs = {}
+        for n in names:   # every solve of the run before its LM runs: b200_lm_solve leaves its own Jacobian on the handle
+            t = time.perf_counter()
+            cs.plan_sparse_schur(rp.C, rp.P, rp.row_cam, rp.row_pt, ORDERINGS[n])
+            analysis_ms = 1e3 * (time.perf_counter() - t)
+            gpu.set_linear_solver_ordering_type(ORDERINGS[n])
+            x, term, ms, kernels = timed_solves(gpu, gpu.sparse_schur_solve, res, D, reps)
+            xs[n] = x
+            out[n]["runs"].append(dict(analysis_ms=round(analysis_ms, 2), solve_ms=round(ms, 3),
+                                       factor_ms=kernels.get("sparse_factor"), termination=int(term)))
+        for n in names:
+            r = out[n]["runs"][-1]
+            if "amd" in xs:
+                r["relerr_vs_amd"] = float(np.linalg.norm(xs[n] - xs["amd"]) / np.linalg.norm(xs["amd"]))
+            # the handle at the call's type: a b200_lm_solve call of another type would analyse again at each call
+            gpu.set_linear_solver_ordering_type(ORDERINGS[n])
+            lm = lm_rate(gpu, state, cs.SPARSE_SCHUR, iterations, linear_solver_ordering_type=ORDERINGS[n])
+            dl = lm_rate(gpu, state, cs.SPARSE_SCHUR, iterations, cs.DOGLEG, cs.TRADITIONAL_DOGLEG,
+                         linear_solver_ordering_type=ORDERINGS[n])
+            r.update(lm_its_per_s=round(lm["its_per_s"], 2), lm_cost=lm["cost"],
+                     dogleg_its_per_s=round(dl["its_per_s"], 2), dogleg_cost=dl["cost"])
+    gpu.set_linear_solver_ordering_type(cs.AMD)
+    for n in names:
+        for key in ("analysis_ms", "solve_ms", "factor_ms", "lm_its_per_s", "dogleg_its_per_s"):
+            v = [r[key] for r in out[n]["runs"] if r.get(key) is not None]
+            if v:
+                out[n][key] = dict(median=float(np.median(v)), min=min(v), max=max(v))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -123,6 +172,8 @@ def main():
     ap.add_argument("--problems", default=",".join(PROBLEMS))
     ap.add_argument("--strategies", default=",".join(n for n, _, _ in STRATEGIES))
     ap.add_argument("--precision", action="store_true")
+    ap.add_argument("--ordering", default=None)
+    ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     device = card()
@@ -141,6 +192,13 @@ def main():
         gpu.scale_columns(s)
         D = np.sqrt(np.clip(gpu.squared_column_norm(), 1e-6, 1e32) / 1e4)
         row = dict(problem=name, device=device, C=rp.C, P=rp.P, N=rp.N, analysis_ms=round(analysis_ms, 2), **st)
+        if a.ordering:
+            row["ordering"] = ordering_axis(gpu, rp, state, res, D, a.ordering.split(","), a.runs, a.reps, a.lm_iterations)
+            row["lm_its_per_s_dense"] = round(lm_rate(gpu, state, cs.DENSE_SCHUR, a.lm_iterations)["its_per_s"], 2)
+            gpu.close()
+            print(json.dumps(row), flush=True)
+            results.append(row)
+            continue
         if a.precision:
             row["precision"] = precision_axis(gpu, state, res, D, a.reps, a.lm_iterations)
             gpu.close()
