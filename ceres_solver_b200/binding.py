@@ -30,7 +30,8 @@ AMD, NESDIS = 0, 1                                  # linear_solver_ordering_typ
 SPARSE_STATS = ("s_blocks", "l_blocks", "l_blocks_caller", "l_blocks_min_degree", "flops_caller", "flops_min_degree",
                 "supernodes", "tree_height", "order", "factor_bytes", "flops", "critical_path_supernodes",
                 "critical_path_flops")
-LOSS_TRIVIAL, LOSS_HUBER = 0, 1
+# B200_LOSS_*, in the order of include/ceres/loss_function.h
+LOSS_TRIVIAL, LOSS_HUBER, LOSS_SOFT_L_ONE, LOSS_CAUCHY, LOSS_ARCTAN, LOSS_TOLERANT, LOSS_TUKEY = range(7)
 
 
 class B200Error(RuntimeError):
@@ -44,6 +45,11 @@ class BaDesc(C.Structure):
                 ("cam_idx", _ip), ("pt_idx", _ip), ("obs", _dp), ("loss_type", C.c_int32), ("loss_a", C.c_double),
                 ("device", C.c_int32), ("stream", C.c_void_p), ("rank", C.c_int32), ("world_size", C.c_int32),
                 ("nccl_unique_id", C.c_void_p)]
+
+
+class Loss(C.Structure):
+    """b200_loss: one loss object; a, b its constructor arguments (only TolerantLoss reads b), scale ScaledLoss's factor."""
+    _fields_ = [("type", C.c_int32), ("a", C.c_double), ("b", C.c_double), ("scale", C.c_double)]
 
 
 class SolverOptions(C.Structure):
@@ -86,7 +92,7 @@ class KernelStat(C.Structure):
 # Every symbol include/b200ba.h declares (tests/test_abi.py checks the library exports all of them).
 SYMBOLS = [
     "b200_plan_point_order", "b200_plan_sparse_schur", "b200_plan_sparse_schur_ordered", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
-    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_plus", "b200_jacobian_squared_column_norm",
+    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_set_loss_functions", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
     "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options",
@@ -219,6 +225,18 @@ class Problem:
 
     def set_apply_loss_function(self, apply):
         _check(lib().b200_set_apply_loss_function(self.h, int(bool(apply))))
+
+    def set_loss_functions(self, losses, row_loss=None):
+        """b200_set_loss_functions: `losses` is a sequence of (type, a, b, scale) tuples (or Loss structures), the table of
+        loss objects; `row_loss` the table index of each row, in this problem's row order (None: every row uses losses[0],
+        which needs exactly one loss)."""
+        table = (Loss * max(1, len(losses)))()
+        for k, l in enumerate(losses):
+            table[k] = l if isinstance(l, Loss) else Loss(*(int(l[0]),) + tuple(float(v) for v in l[1:]))
+        rows = None if row_loss is None else np.ascontiguousarray(row_loss, dtype=np.int32)
+        if rows is not None and rows.size != self.N:
+            raise ValueError("row_loss has %d entries for %d rows" % (rows.size, self.N))
+        _check(lib().b200_set_loss_functions(self.h, table, len(losses), None if rows is None else rows.ctypes.data_as(_ip)))
 
     # ---- Jacobian as a SparseMatrix
     def squared_column_norm(self):

@@ -194,8 +194,14 @@ struct b200_handle {
   int sm_count = 132;
   int C = 0, P = 0, N = 0, num_tiles = 0;
   int np = 0;  // 3P + 9C
-  int loss_type = 0;
-  double loss_a = 1.0;
+  // the loss of every row (b200_create's descriptor or b200_set_loss_functions): its class picks the evaluate instantiation
+  // (loss.cuh); a table of more than one loss object is read per row from d_loss_table through d_row_loss
+  int loss_cls = kLossTrivial;
+  LossEntry loss_one{};
+  int* d_row_loss = nullptr;             // [N], internal row order; allocated by the first table
+  LossEntry* d_loss_table = nullptr;
+  size_t loss_table_cap = 0;
+  bool loss_rows = false;                // the evaluations read d_row_loss and d_loss_table
   bool apply_loss = true;   // EvaluateOptions::apply_loss_function
   int rank = 0, world = 1;
 #ifdef B200_WITH_NCCL
@@ -220,6 +226,7 @@ struct b200_handle {
   // internal point order (b200_create): identity unless `permuted`
   bool permuted = false;
   int *d_pt_perm = nullptr, *d_row_perm = nullptr;   // internal block -> caller block
+  std::vector<int> h_row_perm;                        // ... of the rows, for b200_set_loss_functions
   double *d_stage_p = nullptr, *d_stage_r = nullptr; // boundary staging: [3P+9C], [2N]
   std::vector<int> h_pt_perm;
   bool schur_ready = false;
@@ -490,6 +497,60 @@ int huge_grid(const b200_handle* h) { return std::max(1, std::min(h->num_huge, h
 // ------------------------------------------------------------------------------------------------ device-pointer cores
 int sqnorm_dev(b200_handle* h, double* d_out);
 
+// The evaluate kernels of the plan for one class of loss set (loss.cuh); *num_partials = the per-tile / per-CTA cost
+// partials they wrote.
+template <int kLoss>
+int evaluate_launch(b200_handle* h, EvalArgs a, const double* d_gradient, bool want_jacobian, double* d_sqnorm,
+                    bool* sqnorm_done, int* num_partials) {
+  const bool with_j = want_jacobian || d_gradient != nullptr;
+  const size_t coff = 3 * static_cast<size_t>(h->P);
+  const size_t smem = tile_smem_bytes<3, 1>();
+  *num_partials = h->num_tiles;
+  if (with_j && is_v4(h->mul)) {
+    EvalV2Args e{};
+    e.state = a.state;
+    e.residuals = a.residuals;
+    e.gradient = a.gradient;
+    e.sqnorm = d_sqnorm;
+    e.cost_partial = h->d_tile_partial;
+    e.scale = a.scale;
+    e.fail_flag = h->d_fail;
+    e.loss = a.loss;
+    if (d_sqnorm != nullptr) CU(cudaMemsetAsync(d_sqnorm + coff, 0, sizeof(double) * 9 * h->C, h->stream));
+    if (d_sqnorm != nullptr) OK(huge_zero(h, d_sqnorm));
+    OK(launch(h, K_EVAL_JAC, [&] {
+      if (want_jacobian) evaluate_v2_kernel<kLoss, true><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
+      else evaluate_v2_kernel<kLoss, false><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
+    }));
+    *num_partials = h->v2.num_ctas;
+    if (h->num_big_tiles > 0) {  // the few >32-row points: CTA-tile kernels on their tiles only
+      a.cost_partial = h->d_tile_partial + *num_partials;
+      OK(launch(h, K_EVAL_JAC, [&] {
+        const int grid = std::min(h->num_big_tiles, h->sm_count * 2);
+        if (want_jacobian) evaluate_kernel<kLoss, true><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
+        else evaluate_kernel<kLoss, true, false><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
+      }, false));
+      *num_partials += h->num_big_tiles;
+      if (d_sqnorm != nullptr)
+        OK(launch(h, K_SQNORM, [&] {
+          sqnorm_kernel<<<std::min(h->num_big_tiles, h->sm_count * 4), kTile, tile_smem_bytes<3, 1>(), h->stream>>>(h->view_big, d_sqnorm);
+        }, false));
+    }
+    if (d_sqnorm != nullptr) {
+      OK(allreduce_sum(h, d_sqnorm + coff, 9 * static_cast<size_t>(h->C)));
+      if (sqnorm_done != nullptr) *sqnorm_done = true;
+    }
+  } else if (with_j) {
+    OK(launch(h, K_EVAL_JAC, [&] {
+      if (want_jacobian) evaluate_kernel<kLoss, true><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
+      else evaluate_kernel<kLoss, true, false><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
+    }));
+  } else {
+    OK(launch(h, K_EVAL_COST, [&] { evaluate_kernel<kLoss, false><<<h->grid_tile[K_EVAL_COST], kTile, smem, h->stream>>>(h->view, a); }));
+  }
+  return B200_OK;
+}
+
 // d_sqnorm (optional): squared column norms of the Jacobian as written (after the fused scaling), for free with the
 // warp-tile kernel; the caller falls back to sqnorm_dev when *sqnorm_done comes back false.
 // J is computed (and checked) when the Jacobian or the gradient is asked for, and stored only when want_jacobian: a
@@ -505,58 +566,20 @@ int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, dou
   a.cost_partial = h->d_tile_partial;
   a.scale = d_scale;
   a.fail_flag = h->d_fail;
-  a.loss_type = h->apply_loss ? h->loss_type : B200_LOSS_TRIVIAL;
-  a.loss_a = h->loss_a;
+  a.loss.one = h->loss_one;
+  if (h->loss_rows) {
+    a.loss.row_loss = h->d_row_loss;
+    a.loss.table = h->d_loss_table;
+  }
   if (sqnorm_done != nullptr) *sqnorm_done = false;
   CU(cudaMemsetAsync(h->d_fail, 0, sizeof(int), h->stream));
-  const bool with_j = want_jacobian || d_gradient != nullptr;
-  const size_t coff = 3 * static_cast<size_t>(h->P);
-  if (d_gradient != nullptr) CU(cudaMemsetAsync(d_gradient + coff, 0, sizeof(double) * 9 * h->C, h->stream));
+  if (d_gradient != nullptr) CU(cudaMemsetAsync(d_gradient + 3 * static_cast<size_t>(h->P), 0, sizeof(double) * 9 * h->C, h->stream));
   if (d_gradient != nullptr) OK(huge_zero(h, d_gradient));
-  const size_t smem = tile_smem_bytes<3, 1>();
-  int num_partials = h->num_tiles;
-  if (with_j && is_v4(h->mul)) {
-    EvalV2Args e{};
-    e.state = d_state;
-    e.residuals = d_residuals;
-    e.gradient = d_gradient;
-    e.sqnorm = d_sqnorm;
-    e.cost_partial = h->d_tile_partial;
-    e.scale = d_scale;
-    e.fail_flag = h->d_fail;
-    e.loss_type = a.loss_type;
-    e.loss_a = h->loss_a;
-    if (d_sqnorm != nullptr) CU(cudaMemsetAsync(d_sqnorm + coff, 0, sizeof(double) * 9 * h->C, h->stream));
-    if (d_sqnorm != nullptr) OK(huge_zero(h, d_sqnorm));
-    OK(launch(h, K_EVAL_JAC, [&] {
-      if (want_jacobian) evaluate_v2_kernel<true><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
-      else evaluate_v2_kernel<false><<<h->v2.num_ctas, 32 * h->v2.warps, h->eval_v2_smem, h->stream>>>(h->v2_eval, e);
-    }));
-    num_partials = h->v2.num_ctas;
-    if (h->num_big_tiles > 0) {  // the few >32-row points: CTA-tile kernels on their tiles only
-      a.cost_partial = h->d_tile_partial + num_partials;
-      OK(launch(h, K_EVAL_JAC, [&] {
-        const int grid = std::min(h->num_big_tiles, h->sm_count * 2);
-        if (want_jacobian) evaluate_kernel<true><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
-        else evaluate_kernel<true, false><<<grid, kTile, smem, h->stream>>>(h->view_big, a);
-      }, false));
-      num_partials += h->num_big_tiles;
-      if (d_sqnorm != nullptr)
-        OK(launch(h, K_SQNORM, [&] {
-          sqnorm_kernel<<<std::min(h->num_big_tiles, h->sm_count * 4), kTile, tile_smem_bytes<3, 1>(), h->stream>>>(h->view_big, d_sqnorm);
-        }, false));
-    }
-    if (d_sqnorm != nullptr) {
-      OK(allreduce_sum(h, d_sqnorm + coff, 9 * static_cast<size_t>(h->C)));
-      if (sqnorm_done != nullptr) *sqnorm_done = true;
-    }
-  } else if (with_j) {
-    OK(launch(h, K_EVAL_JAC, [&] {
-      if (want_jacobian) evaluate_kernel<true><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
-      else evaluate_kernel<true, false><<<h->grid_tile[K_EVAL_JAC], kTile, smem, h->stream>>>(h->view, a);
-    }));
-  } else {
-    OK(launch(h, K_EVAL_COST, [&] { evaluate_kernel<false><<<h->grid_tile[K_EVAL_COST], kTile, smem, h->stream>>>(h->view, a); }));
+  int num_partials = 0;
+  switch (h->apply_loss ? h->loss_cls : kLossTrivial) {
+    case kLossTrivial: OK(evaluate_launch<kLossTrivial>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
+    case kLossHuber: OK(evaluate_launch<kLossHuber>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
+    default: OK(evaluate_launch<kLossGeneral>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
   }
   OK(launch(h, K_MISC, [&] { sum_kernel<<<1, kVecThreads, 0, h->stream>>>(num_partials, h->d_tile_partial, h->d_scalars); }));
   if (d_gradient != nullptr) OK(allreduce_sum(h, d_gradient + 3 * static_cast<size_t>(h->P), 9 * static_cast<size_t>(h->C)));
@@ -1593,8 +1616,12 @@ int set_func_attributes(int smem_optin) {
   OK(raise_smem_limit(jtj_v4_kernel<false>, lim));
   OK(raise_smem_limit(schur_mul_v4_kernel<true>, lim));
   OK(raise_smem_limit(schur_mul_v4_kernel<false>, lim));
-  OK(raise_smem_limit(evaluate_v2_kernel<true>, lim));
-  OK(raise_smem_limit(evaluate_v2_kernel<false>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossTrivial, true>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossTrivial, false>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossHuber, true>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossHuber, false>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossGeneral, true>, lim));
+  OK(raise_smem_limit(evaluate_v2_kernel<kLossGeneral, false>, lim));
   OK(raise_smem_limit(diag_blocks_v2_kernel<true>, lim));
   OK(raise_smem_limit(diag_blocks_v2_kernel<false>, lim));
   OK(raise_smem_limit(xs_pcg_kernel, lim));
@@ -2251,6 +2278,9 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   if (desc->num_observations > 2000000000LL) return fail(B200_ERR_UNSUPPORTED, "more than 2e9 row blocks");
   if (desc->cam_idx == nullptr || desc->pt_idx == nullptr || desc->obs == nullptr)
     return fail(B200_ERR_INVALID_ARGUMENT, "null structure array");
+  if (desc->loss_type != B200_LOSS_TRIVIAL && desc->loss_type != B200_LOSS_HUBER)
+    return fail(B200_ERR_INVALID_ARGUMENT, "loss_type %d: the descriptor takes B200_LOSS_TRIVIAL or B200_LOSS_HUBER, other losses "
+                "go through b200_set_loss_functions", desc->loss_type);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
@@ -2292,8 +2322,11 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   h->N = N;
   h->np = 3 * P + 9 * C;
   h->num_tiles = static_cast<int>(pl.tiles.size());
-  h->loss_type = desc->loss_type;
-  h->loss_a = desc->loss_a;
+  h->loss_one.type = desc->loss_type;
+  h->loss_one.p = desc->loss_a;
+  h->loss_one.q = desc->loss_a * desc->loss_a;
+  h->loss_one.scale = 1.0;
+  h->loss_cls = desc->loss_type == B200_LOSS_HUBER ? kLossHuber : kLossTrivial;
   h->rank = world > 1 ? desc->rank : 0;
   h->world = world;
   h->knobs = knobs;
@@ -2358,6 +2391,7 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
     OK(dev_alloc(h, &h->d_stage_p, h->np));
     OK(dev_alloc(h, &h->d_stage_r, 2 * n));
     h->h_pt_perm = pl.pt_perm;
+    h->h_row_perm = pl.row_perm;
     h->permuted = true;
   }
   if (h->diag == DiagPass::CamMajor) {
@@ -2468,8 +2502,10 @@ int b200_create(const b200_ba_desc* desc, b200_handle** out) {
   }
 
   for (int k = 0; k < K_COUNT; ++k) h->grid_tile[k] = std::max(1, std::min(h->num_tiles, h->sm_count * 4));
-  h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<true>, tile_smem_bytes<3, 1>());
-  h->grid_tile[K_EVAL_COST] = tile_grid(h, evaluate_kernel<false>, tile_smem_bytes<3, 1>());
+  // (from the Huber instantiations, which use the most registers of the trivial and Huber ones; the persistent tile loop
+  // is correct at any grid)
+  h->grid_tile[K_EVAL_JAC] = tile_grid(h, evaluate_kernel<kLossHuber, true>, tile_smem_bytes<3, 1>());
+  h->grid_tile[K_EVAL_COST] = tile_grid(h, evaluate_kernel<kLossHuber, false>, tile_smem_bytes<3, 1>());
   h->grid_tile[K_SQNORM] = tile_grid(h, sqnorm_kernel, tile_smem_bytes<3, 1>());
   h->grid_tile[K_JMUL] = tile_grid(h, jmul_kernel, tile_smem_bytes<1, 1>());
   h->grid_tile[K_JTMUL] = tile_grid(h, jtmul_kernel<false>, tile_smem_bytes<3, 1>());
@@ -2614,6 +2650,72 @@ int b200_evaluate(b200_handle* h, const double* state, double* cost, double* res
 int b200_set_apply_loss_function(b200_handle* h, int apply) {
   if (h == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
   h->apply_loss = apply != 0;
+  return B200_OK;
+}
+
+namespace {
+// A loss object as the kernels read it (loss.cuh LossEntry), with the checks of its constructor; false if it is refused.
+bool make_loss_entry(const b200_loss& l, LossEntry* e) {
+  const double a = l.a, b = l.b;
+  *e = LossEntry{};
+  e->type = l.type;
+  e->scale = l.scale;
+  if (!std::isfinite(l.scale) || l.scale <= 0.0) return false;
+  switch (l.type) {
+    case B200_LOSS_TRIVIAL:
+      return true;
+    case B200_LOSS_TOLERANT:
+      if (!std::isfinite(a) || !std::isfinite(b) || a < 0.0 || b <= 0.0) return false;
+      e->p = a;
+      e->q = b;
+      e->r = b * std::log(1.0 + std::exp(-a / b));
+      return true;
+    case B200_LOSS_HUBER: case B200_LOSS_SOFT_L_ONE: case B200_LOSS_CAUCHY: case B200_LOSS_ARCTAN: case B200_LOSS_TUKEY:
+      if (!std::isfinite(a) || a <= 0.0) return false;
+      e->p = a;
+      e->q = l.type == B200_LOSS_ARCTAN ? 1.0 / (a * a) : a * a;
+      e->r = 1.0 / (a * a);
+      return true;
+    default:
+      return false;
+  }
+}
+}  // namespace
+
+int b200_set_loss_functions(b200_handle* h, const b200_loss* losses, int num_losses, const int32_t* row_loss) {
+  if (h == nullptr || losses == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  if (num_losses < 1) return fail(B200_ERR_INVALID_ARGUMENT, "num_losses %d < 1", num_losses);
+  if (row_loss == nullptr && num_losses != 1) return fail(B200_ERR_INVALID_ARGUMENT, "row_loss == NULL needs one loss, not %d", num_losses);
+  std::vector<LossEntry> table(num_losses);
+  for (int k = 0; k < num_losses; ++k)
+    if (!make_loss_entry(losses[k], &table[k]))
+      return fail(B200_ERR_INVALID_ARGUMENT, "loss %d: type %d, a %g, b %g, scale %g refused", k, losses[k].type, losses[k].a,
+                  losses[k].b, losses[k].scale);
+  if (row_loss != nullptr)
+    for (int i = 0; i < h->N; ++i)
+      if (row_loss[i] < 0 || row_loss[i] >= num_losses)
+        return fail(B200_ERR_INVALID_ARGUMENT, "row %d: loss index %d outside [0, %d)", i, row_loss[i], num_losses);
+  CU(cudaSetDevice(h->device));
+  const bool rows = num_losses > 1;   // one loss object, indexed or not, is every row's: no per-row array
+  if (rows) {
+    std::vector<int> internal(h->N);
+    for (int i = 0; i < h->N; ++i) internal[i] = row_loss[h->permuted ? h->h_row_perm[i] : i];
+    if (h->d_row_loss == nullptr) OK(dev_alloc(h, &h->d_row_loss, h->N));
+    if (h->loss_table_cap < table.size()) {
+      dev_free(h, h->d_loss_table);
+      OK(dev_alloc(h, &h->d_loss_table, table.size()));
+      h->loss_table_cap = table.size();
+    }
+    CU(cudaMemcpyAsync(h->d_row_loss, internal.data(), sizeof(int) * internal.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_loss_table, table.data(), sizeof(LossEntry) * table.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+  }
+  const LossEntry& one = table[0];
+  h->loss_rows = rows;
+  h->loss_one = one;
+  if (rows || one.scale != 1.0) h->loss_cls = kLossGeneral;
+  else h->loss_cls = one.type == B200_LOSS_TRIVIAL ? kLossTrivial : one.type == B200_LOSS_HUBER ? kLossHuber : kLossGeneral;
+  h->residuals_resident = false;   // they were corrected by the previous losses
   return B200_OK;
 }
 

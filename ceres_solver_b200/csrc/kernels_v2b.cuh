@@ -93,8 +93,7 @@ struct EvalV2Args {
   double* cost_partial;  // [num_ctas]
   const double* scale;   // null or [3P+9C]
   int* fail_flag;
-  int loss_type;
-  double loss_a;
+  LossArgs loss;
 };
 
 constexpr int kEvalScratch = 3;  // doubles per lane in the exchange scratch
@@ -102,8 +101,8 @@ __host__ __device__ inline int eval_v2_per_warp_bytes() { return 32 * 144 + 32 *
 
 // Evaluate residuals, Jacobian (written through a per-warp staging buffer + TMA bulk store), cost, gradient and the
 // squared column norms of the Jacobian as written (i.e. after the fused Jacobi scaling).
-// kStoreJ = false (gradient without the Jacobian): as evaluate_kernel<true, false>, the Jacobian is left as it is.
-template <bool kStoreJ>
+// kStoreJ = false (gradient without the Jacobian): as evaluate_kernel<kLoss, true, false>, the Jacobian is left as it is.
+template <int kLoss, bool kStoreJ>
 __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v, EvalV2Args a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -149,56 +148,7 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
 #pragma unroll
       for (int k = 0; k < 6; ++k) finite = finite && isfinite(jp[k]);
       if (!finite) atomicExch(a.fail_flag, 1);
-      const double sq = r0 * r0 + r1 * r1;
-      if (a.loss_type == 0) {
-        cost += 0.5 * sq;
-      } else {
-        const double b = a.loss_a * a.loss_a;
-        double rho0, rho1, rho2;
-        if (sq > b) {
-          const double rr = sqrt(sq);
-          rho0 = 2.0 * a.loss_a * rr - b;
-          rho1 = fmax(2.2250738585072014e-308, a.loss_a / rr);
-          rho2 = -rho1 / (2.0 * sq);
-        } else {
-          rho0 = sq;
-          rho1 = 1.0;
-          rho2 = 0.0;
-        }
-        cost += 0.5 * rho0;
-        const double sqrt_rho1 = sqrt(rho1);
-        double residual_scaling, alpha_sq_norm;
-        if (sq == 0.0 || rho2 <= 0.0) {
-          residual_scaling = sqrt_rho1;
-          alpha_sq_norm = 0.0;
-        } else {
-          const double Dd = 1.0 + 2.0 * sq * rho2 / rho1;
-          const double alpha = 1.0 - sqrt(Dd);
-          residual_scaling = sqrt_rho1 / (1.0 - alpha);
-          alpha_sq_norm = alpha / sq;
-        }
-        if (alpha_sq_norm == 0.0) {
-#pragma unroll
-          for (int k = 0; k < 18; ++k) jc[k] *= sqrt_rho1;
-#pragma unroll
-          for (int k = 0; k < 6; ++k) jp[k] *= sqrt_rho1;
-        } else {
-#pragma unroll
-          for (int k = 0; k < 9; ++k) {
-            const double rtj = jc[k] * r0 + jc[9 + k] * r1;
-            jc[k] = sqrt_rho1 * (jc[k] - alpha_sq_norm * r0 * rtj);
-            jc[9 + k] = sqrt_rho1 * (jc[9 + k] - alpha_sq_norm * r1 * rtj);
-          }
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            const double rtj = jp[k] * r0 + jp[3 + k] * r1;
-            jp[k] = sqrt_rho1 * (jp[k] - alpha_sq_norm * r0 * rtj);
-            jp[3 + k] = sqrt_rho1 * (jp[3 + k] - alpha_sq_norm * r1 * rtj);
-          }
-        }
-        r0 *= residual_scaling;
-        r1 *= residual_scaling;
-      }
+      cost += apply_loss<kLoss, true>(row_loss_entry<kLoss>(a.loss, row), r0, r1, jc, jp);
       if (a.residuals != nullptr) *reinterpret_cast<double2*>(a.residuals + 2 * row) = make_double2(r0, r1);
     }
     // gradient of the unscaled Jacobian (program_evaluator.h:242-259)
