@@ -92,7 +92,7 @@ class KernelStat(C.Structure):
 # Every symbol include/b200ba.h declares (tests/test_abi.py checks the library exports all of them).
 SYMBOLS = [
     "b200_plan_point_order", "b200_plan_sparse_schur", "b200_plan_sparse_schur_ordered", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
-    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_set_loss_functions", "b200_plus", "b200_jacobian_squared_column_norm",
+    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_set_loss_functions", "b200_set_constant_blocks", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
     "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options",
@@ -237,6 +237,21 @@ class Problem:
         if rows is not None and rows.size != self.N:
             raise ValueError("row_loss has %d entries for %d rows" % (rows.size, self.N))
         _check(lib().b200_set_loss_functions(self.h, table, len(losses), None if rows is None else rows.ctypes.data_as(_ip)))
+
+    def set_constant_blocks(self, camera_constant=None, point_constant=None):
+        """b200_set_constant_blocks: boolean arrays of C cameras and of this problem's P points (True = constant); None =
+        none.  Replaces the problem's set (Problem::SetParameterBlockConstant / SetParameterBlockVariable)."""
+        flags = []
+        for a, n, what in ((camera_constant, self.C, "camera_constant"), (point_constant, self.P, "point_constant")):
+            if a is None:
+                flags.append(None)
+                continue
+            a = np.ascontiguousarray(np.asarray(a).astype(bool).astype(np.uint8))
+            if a.size != n:
+                raise ValueError("%s has %d entries for %d blocks" % (what, a.size, n))
+            flags.append(a)
+        _check(lib().b200_set_constant_blocks(self.h, *(None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
+                                                       for a in flags)))
 
     # ---- Jacobian as a SparseMatrix
     def squared_column_norm(self):

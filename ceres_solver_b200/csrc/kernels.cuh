@@ -133,6 +133,18 @@ __device__ __forceinline__ void snavely(const double* __restrict__ cam, double X
   }
 }
 
+// Zeroes a row's cells of its constant blocks: jp when the point (component po) is constant, jc when the camera (pc) is.
+__device__ __forceinline__ void fixed_cells(const uint8_t* __restrict__ fixed, size_t po, size_t pc, double* jc, double* jp) {
+  if (__ldg(fixed + po) != 0) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) jp[k] = 0.0;
+  }
+  if (__ldg(fixed + pc) != 0) {
+#pragma unroll
+    for (int k = 0; k < 18; ++k) jc[k] = 0.0;
+  }
+}
+
 struct EvalArgs {
   const double* state;   // [3P+9C]
   double* residuals;     // [2N] or null
@@ -141,12 +153,16 @@ struct EvalArgs {
   const double* scale;   // null or [3P+9C]: Jacobi scaling fused into the Jacobian write (J <- J diag(scale))
   int* fail_flag;        // set to 1 on a non-finite residual/Jacobian entry
   LossArgs loss;
+  const uint8_t* fixed;  // [3P+9C], read with kFixed only: nonzero on the components of constant blocks
 };
 
 // kStoreJ = false (gradient without the Jacobian): J is computed, checked and used for the gradient, but the stored
 // Jacobian is left as it is.  A template parameter, so that the instantiation the LM loop runs is the same code.
 // kLoss: the class of the handle's loss set (loss.cuh).
-template <int kLoss, bool kWantJ, bool kStoreJ = kWantJ>
+// kFixed: the handle holds blocks constant.  Their cells are set to 0 before anything reads them: they are not checked
+// for finiteness, not corrected by the loss, and stored, summed into the gradient and scaled as 0 (the columns
+// Program::RemoveFixedBlocks leaves out of the reduced program).
+template <int kLoss, bool kWantJ, bool kStoreJ = kWantJ, bool kFixed = false>
 __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const TileSmem s = carve_smem<3, 1>(smem_raw);
@@ -168,6 +184,7 @@ __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs
       const double* cp = a.state + 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(cam);
       const double2 o = *reinterpret_cast<const double2*>(p.obs + 2 * row);
       snavely<kWantJ>(cp, X[0], X[1], X[2], o.x, o.y, r0, r1, jc, jp);
+      if (kFixed && kWantJ) fixed_cells(a.fixed, 3 * static_cast<size_t>(d.pt_begin + lpt), 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(cam), jc, jp);
       bool finite = isfinite(r0) && isfinite(r1);
       if (kWantJ) {
 #pragma unroll
@@ -300,6 +317,23 @@ __global__ void __launch_bounds__(kTile) sqnorm_kernel(ProblemView p, double* ou
       }
     }
     __syncthreads();
+  }
+}
+
+// Zeroes the stored cells of constant blocks (fixed: [3P+9C], nonzero on their components): the E cells of rows whose point
+// is constant, the F cells of rows whose camera is.  Same flat walk as scale_kernel.
+__global__ void __launch_bounds__(256) fixed_mask_kernel(ProblemView p, const uint8_t* __restrict__ fixed) {
+  const size_t nE2 = 3 * static_cast<size_t>(p.N), nF2 = 9 * static_cast<size_t>(p.N);
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  double2* E2 = reinterpret_cast<double2*>(p.E());
+  double2* F2 = reinterpret_cast<double2*>(p.F());
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nE2 + nF2; i += stride) {
+    if (i < nE2) {
+      if (fixed[3 * static_cast<size_t>(p.pt_of_row[i / 3])] != 0) E2[i] = make_double2(0.0, 0.0);
+    } else {
+      const size_t j = i - nE2;
+      if (fixed[3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(p.cam_idx[j / 9])] != 0) F2[j] = make_double2(0.0, 0.0);
+    }
   }
 }
 

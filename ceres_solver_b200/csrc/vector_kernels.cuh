@@ -47,6 +47,14 @@ __global__ void __launch_bounds__(256) fill_kernel(size_t n, double* y, double v
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) y[i] = v;
 }
 
+// D' of the solves on a handle with constant blocks: 1 on their components, D (0 when null) elsewhere.  Their E'E + D'^2
+// and S blocks are then identities decoupled from the rest, and the solves return exact zeros there.
+__global__ void __launch_bounds__(256) solve_diagonal_kernel(int n, const double* __restrict__ D, const uint8_t* __restrict__ fixed,
+                                                             double* out) {
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = fixed[i] != 0 ? 1.0 : D != nullptr ? D[i] : 0.0;
+}
+
 // ---------------------------------------------------------------- LM vector kernels (n = 3P+9C)
 // scale = 1 / (1 + sqrt(colnorm^2))     trust_region_minimizer.cc:263-274
 __global__ void __launch_bounds__(256) jacobi_scale_kernel(int n, const double* __restrict__ sqnorm, double* scale) {
@@ -76,9 +84,11 @@ __global__ void __launch_bounds__(256) lm_diagonal_kernel(int n, int refresh, co
 // Generic two-stage deterministic reductions: partial[blockIdx.x*kSlots + s], then reduce_final_kernel.
 constexpr int kRedBlocks = 296;
 // step = -y ; delta = step*scale ; cand = x + delta ; partials: {|delta|^2, |x|^2, nonfinite count}
+// fixed: null, or nonzero on the components of constant blocks: cand = x there, and |x|^2 is taken over the variable
+// components only, as over Ceres' reduced x (trust_region_minimizer.cc:725-742).
 __global__ void __launch_bounds__(256)
     lm_step_kernel(int n, const double* __restrict__ y, const double* __restrict__ scale, const double* __restrict__ x,
-                   double* step, double* cand, double* partial) {
+                   const uint8_t* __restrict__ fixed, double* step, double* cand, double* partial) {
   __shared__ double scratch[32];
   double a = 0.0, b = 0.0, c = 0.0;
   const int stride = gridDim.x * blockDim.x;
@@ -88,11 +98,12 @@ __global__ void __launch_bounds__(256)
     step[i] = si;
     const double di = si * scale[i];
     const double xi = x[i];
-    const double ci = xi + di;
+    const bool fx = fixed != nullptr && fixed[i] != 0;
+    const double ci = fx ? xi : xi + di;
     cand[i] = ci;
     const double dd = xi - ci;
     a += dd * dd;
-    b += xi * xi;
+    if (!fx) b += xi * xi;
     if (!isfinite(yi)) c += 1.0;
   }
   a = block_sum<256>(a, scratch);
@@ -178,10 +189,12 @@ __global__ void __launch_bounds__(256) dogleg_gn_kernel(int n, const double* __r
 // The dogleg step (dogleg.h StepKind): v = gn (kind 0), cg g (kind 1) or cg g + cn gn (kind 2), selected rather than
 // multiplied by 0; step = v / diagonal; delta = step * scale; cand = x + delta.
 // Partials {|x - cand|^2, |x|^2, non-finite step count, |v|^2 (dogleg_step_norm_ of the interpolation, :251)}.
+// fixed: as in lm_step_kernel.
 __global__ void __launch_bounds__(256)
     dogleg_step_kernel(int n, int kind, double cg, double cn, const double* __restrict__ g, const double* __restrict__ gn,
                        const double* __restrict__ diagonal, const double* __restrict__ scale,
-                       const double* __restrict__ x, double* step, double* cand, double* partial) {
+                       const double* __restrict__ x, const uint8_t* __restrict__ fixed, double* step, double* cand,
+                       double* partial) {
   __shared__ double scratch[32];
   double a = 0.0, b = 0.0, c = 0.0, e = 0.0;
   const int stride = gridDim.x * blockDim.x;
@@ -193,11 +206,12 @@ __global__ void __launch_bounds__(256)
     const double si = v / diagonal[i];
     step[i] = si;
     const double xi = x[i];
-    const double ci = __dadd_rn(xi, __dmul_rn(si, scale[i]));
+    const bool fx = fixed != nullptr && fixed[i] != 0;
+    const double ci = fx ? xi : __dadd_rn(xi, __dmul_rn(si, scale[i]));
     cand[i] = ci;
     const double dd = xi - ci;
     a = __fma_rn(dd, dd, a);
-    b = __fma_rn(xi, xi, b);
+    if (!fx) b = __fma_rn(xi, xi, b);
     if (!isfinite(si)) c += 1.0;
     e = __fma_rn(v, v, e);
   }

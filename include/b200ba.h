@@ -171,6 +171,28 @@ int b200_set_apply_loss_function(b200_handle* h, int apply);
  * scale or scale <= 0, a non-finite a or a <= 0 for Huber, SoftLOne, Cauchy, Arctan and Tukey, and for Tolerant a
  * non-finite a or b, a < 0 or b <= 0 (TolerantLoss's CHECKs). */
 int b200_set_loss_functions(b200_handle* h, const b200_loss* losses, int num_losses, const int32_t* row_loss);
+/* Problem::SetParameterBlockConstant / SetParameterBlockVariable for every block at once.
+   camera_constant[C], point_constant[P]: nonzero = constant. Points are this shard's, in the caller's order.
+   NULL = none.
+ * The call replaces the handle's set; the new set applies from the next evaluation on.  The layout stays [3P | 9C] and
+ * b200_num_parameters is unchanged: a constant block is handled as Ceres' reduced program handles it
+ * (Program::RemoveFixedBlocks), as Jacobian columns that are exactly zero.
+ *  - Evaluation neither checks nor corrects a constant block's cells (a non-finite value there does not fail it) and
+ *    stores them as 0, so J'r, the column norms and J'x are 0 on its components.
+ *  - The solves (b200_schur_solve, b200_dense_schur_solve, b200_sparse_schur_solve, b200_schur_init) use D' = 1 on the
+ *    constant components and the caller's D (0 for D == NULL) elsewhere: (E'E + D'^2)^-1 and the preconditioner blocks are
+ *    identities on constant blocks, which are decoupled from the others, and every solution, b200_schur_back_substitute's
+ *    included, is 0 there.  The other components are solved as in the reduced program.
+ *  - Inputs on constant components are ignored: b200_plus returns x there; b200_lm_solve reads the state and returns its
+ *    constant blocks bitwise unchanged, and takes |x| for parameter_tolerance over the variable blocks only
+ *    (trust_region_minimizer.cc:725-742).  b200_jtj_multiply adds D^2 x there, as it does for any zero column.
+ *  - The stored Jacobian's cells of the now-constant blocks are zeroed by the call, and b200_jacobian_set_values zeroes
+ *    them after every upload; cells of blocks made variable keep what they held until the next evaluation with J.  The
+ *    explicit S, the Schur initialisation and the preconditioner are invalidated; the resident residuals are kept.
+ *  - Sharded handles: each rank passes its own points' flags and the same camera flags.
+ * B200_ERR_INVALID_ARGUMENT, with the handle unchanged: h == NULL, or a row whose camera and point are both constant
+ * (Ceres moves such a row's cost into fixed_cost; drop the row from the problem, as Program::RemoveFixedBlocks does). */
+int b200_set_constant_blocks(b200_handle* h, const uint8_t* camera_constant, const uint8_t* point_constant);
 /* Evaluator::Plus (evaluator.h:146; Euclidean manifolds only): x_plus_delta = x + delta. */
 int b200_plus(b200_handle* h, const double* x, const double* delta, double* x_plus_delta);
 
