@@ -76,6 +76,12 @@ class LmOptions(C.Structure):
                 ("linear_solver_ordering_type", C.c_int32)]
 
 
+class CovarianceOptions(C.Structure):
+    """b200_covariance_options: Covariance::Options' algorithm_type, min_reciprocal_condition_number, apply_loss_function."""
+    _fields_ = [("algorithm", C.c_int32), ("min_reciprocal_condition_number", C.c_double),
+                ("apply_loss_function", C.c_int32)]
+
+
 class LmIteration(C.Structure):
     _fields_ = [("iteration", C.c_int32), ("linear_solver_iterations", C.c_int32), ("step_is_valid", C.c_int32),
                 ("step_is_successful", C.c_int32), ("cost", C.c_double), ("cost_change", C.c_double),
@@ -99,7 +105,8 @@ SYMBOLS = [
     "b200_set_linear_solver_ordering_type", "b200_schur_init", "b200_schur_rhs", "b200_schur_ete_inverse", "b200_schur_multiply",
     "b200_schur_back_substitute", "b200_schur_jacobi_update", "b200_block_jacobi_update",
     "b200_lm_options_default", "b200_lm_solve", "b200_profile_enable", "b200_stats_reset", "b200_stats_get",
-    "b200_total_launches", "b200_synchronize", "b200_transfer_bytes",
+    "b200_total_launches", "b200_synchronize", "b200_transfer_bytes", "b200_covariance_options_default",
+    "b200_covariance_compute", "b200_covariance_cameras", "b200_covariance_points", "b200_plan_sparse_selinv",
 ]
 
 _lib = None
@@ -160,6 +167,25 @@ def plan_sparse_schur(num_cameras, num_points, cam_idx, pt_idx, ordering_type=AM
     stats = (C.c_int64 * len(SPARSE_STATS))()
     _check(lib().b200_plan_sparse_schur_ordered(C.byref(d), int(ordering_type), perm.ctypes.data_as(_ip), stats))
     return perm, {k: int(v) for k, v in zip(SPARSE_STATS, stats)}
+
+
+def plan_sparse_selinv(num_cameras, num_points, cam_idx, pt_idx, ordering_type=AMD):
+    """Host-only: the selected inversion's task graph for this structure.  Returns (sn_first [ns + 1], order [ns],
+    counter init [ns])."""
+    cam = np.ascontiguousarray(cam_idx, dtype=np.int32)
+    pt = np.ascontiguousarray(pt_idx, dtype=np.int32)
+    d = BaDesc()
+    d.num_cameras, d.num_points, d.num_observations = int(num_cameras), int(num_points), len(cam)
+    d.cam_idx = cam.ctypes.data_as(_ip)
+    d.pt_idx = pt.ctypes.data_as(_ip)
+    ns = C.c_int32()
+    first = np.zeros(int(num_cameras) + 1, dtype=np.int32)
+    order = np.zeros(int(num_cameras), dtype=np.int32)
+    cnt = np.zeros(int(num_cameras), dtype=np.int32)
+    _check(lib().b200_plan_sparse_selinv(C.byref(d), int(ordering_type), C.byref(ns), first.ctypes.data_as(_ip),
+                                         order.ctypes.data_as(_ip), cnt.ctypes.data_as(_ip)))
+    n = ns.value
+    return first[:n + 1].copy(), order[:n].copy(), cnt[:n].copy()
 
 
 def nccl_unique_id():
@@ -374,6 +400,33 @@ class Problem:
         _check(lib().b200_block_jacobi_update(self.h, _d(inv)))
         return inv
 
+    # ---- Covariance
+    def covariance_compute(self, state, algorithm=SPARSE_SCHUR, min_reciprocal_condition_number=1e-14,
+                           apply_loss_function=True):
+        """b200_covariance_compute: Covariance::Compute at `state`; returns its bool (False: not positive definite or
+        worse conditioned than min_reciprocal_condition_number)."""
+        o = CovarianceOptions()
+        lib().b200_covariance_options_default(C.byref(o))
+        o.algorithm = int(algorithm)
+        o.min_reciprocal_condition_number = float(min_reciprocal_condition_number)
+        o.apply_loss_function = int(bool(apply_loss_function))
+        valid = C.c_int()
+        _check(lib().b200_covariance_compute(self.h, _d(_f64(state)), C.byref(o), C.byref(valid)))
+        return bool(valid.value)
+
+    def covariance_cameras(self, pairs):
+        """Cov(c_i, c_j) of each (i, j) in `pairs`: (n, 9, 9), row-major blocks."""
+        p = np.ascontiguousarray(np.asarray(pairs, dtype=np.int32).reshape(-1, 2))
+        out = np.zeros((len(p), 9, 9))
+        _check(lib().b200_covariance_cameras(self.h, len(p), p.ctypes.data_as(_ip), _d(out)))
+        return out
+
+    def covariance_points(self):
+        """Cov(p, p) of every point: (P, 3, 3)."""
+        out = np.zeros((self.P, 3, 3))
+        _check(lib().b200_covariance_points(self.h, _d(out)))
+        return out
+
     # ---- trust region loop
     @staticmethod
     def lm_options(**kw):
@@ -407,9 +460,9 @@ class Problem:
         _check(lib().b200_stats_reset(self.h))
 
     def stats(self):
-        arr = (KernelStat * 32)()
+        arr = (KernelStat * 64)()
         n = C.c_int()
-        _check(lib().b200_stats_get(self.h, arr, 32, C.byref(n)))
+        _check(lib().b200_stats_get(self.h, arr, 64, C.byref(n)))
         return {arr[i].name.decode(): dict(launches=arr[i].launches, operations=arr[i].operations, ms=arr[i].device_ms,
                                            bytes_per_operation=arr[i].bytes_per_operation) for i in range(n.value)}
 

@@ -42,6 +42,7 @@
 #include "plan.cuh"
 #include "sparse_plan.cuh"
 #include "sparse_schur.cuh"
+#include "covariance.cuh"
 #include "dogleg.h"
 
 using namespace b200;
@@ -85,6 +86,8 @@ struct CusolverApi {
   typedef int (*spotrf_bs_t)(void*, int, int, float*, int, int*);
   typedef int (*spotrf_t)(void*, int, int, float*, int, float*, int, int*);
   typedef int (*spotrs_t)(void*, int, int, int, const float*, int, float*, int, int*);
+  typedef int (*potri_bs_t)(void*, int, int, double*, int, int*);
+  typedef int (*potri_t)(void*, int, int, double*, int, double*, int, int*);
   create_t Create = nullptr;
   destroy_t Destroy = nullptr;
   set_stream_t SetStream = nullptr;
@@ -96,7 +99,10 @@ struct CusolverApi {
   spotrf_bs_t SpotrfBufferSize = nullptr;
   spotrf_t Spotrf = nullptr;
   spotrs_t Spotrs = nullptr;
-  bool ok = false, float_ok = false;
+  // the inverse from the factor (b200_covariance_compute with B200_DENSE_SCHUR), bound on its own as well
+  potri_bs_t DpotriBufferSize = nullptr;
+  potri_t Dpotri = nullptr;
+  bool ok = false, float_ok = false, potri_ok = false;
 };
 CusolverApi g_cusolver;
 bool load_cusolver() {
@@ -117,6 +123,9 @@ bool load_cusolver() {
   g_cusolver.Spotrf = reinterpret_cast<CusolverApi::spotrf_t>(dlsym(lib, "cusolverDnSpotrf"));
   g_cusolver.Spotrs = reinterpret_cast<CusolverApi::spotrs_t>(dlsym(lib, "cusolverDnSpotrs"));
   g_cusolver.float_ok = g_cusolver.SpotrfBufferSize && g_cusolver.Spotrf && g_cusolver.Spotrs;
+  g_cusolver.DpotriBufferSize = reinterpret_cast<CusolverApi::potri_bs_t>(dlsym(lib, "cusolverDnDpotri_bufferSize"));
+  g_cusolver.Dpotri = reinterpret_cast<CusolverApi::potri_t>(dlsym(lib, "cusolverDnDpotri"));
+  g_cusolver.potri_ok = g_cusolver.DpotriBufferSize && g_cusolver.Dpotri;
   return g_cusolver.ok;
 }
 
@@ -304,6 +313,27 @@ struct b200_handle {
   int sp_grid = 0, sp_grid32 = 0;
   size_t sp_smem = 0, sp_smem32 = 0;
   int* d_sp_cnt_init = nullptr;
+  int* d_sp_cnt_inv = nullptr;  // [ns] SparsePlan::cnt_inv
+  int sp_selinv_grid = 0;
+  size_t sp_selinv_smem = 0;
+  double sp_selinv_flops = 0.0;
+  // b200_covariance_compute (covariance.cuh): the snapshot the getters read, and the scratch that forms it
+  bool cov_valid = false;
+  int cov_alg = B200_SPARSE_SCHUR;
+  std::vector<int> cov_row_ptr, cov_blk_col;   // S's block pattern (sparse snapshot): block row ptr, block columns
+  std::vector<uint8_t> cov_cam_fixed;          // [C] the constant cameras of the snapshot
+  int* d_cov_row_ptr = nullptr;                // [C + 1]
+  double* d_cov_s = nullptr;                   // sparse: Z on S's blocks [81 x blocks], row-major, S's block order
+  double* d_cov_dense = nullptr;               // dense: S, its factor, then Z's lower triangle [9C][9C]
+  double* d_cov_diag = nullptr;                // dense: S's diagonal before the factorisation [9C]
+  double* d_cov_work = nullptr;
+  int cov_lwork = 0;
+  double* d_cov_z = nullptr;                   // sparse: Z in the factor's panel layout [sp_storage]
+  double* d_cov_pts = nullptr;                 // [9P] Cov(p, p), caller's point order
+  unsigned long long* d_cov_min = nullptr;     // the conditioning test's minimum, as bits, and the dense info
+  int4* d_cov_pairs = nullptr;
+  double* d_cov_out = nullptr;
+  size_t cov_pairs_cap = 0;
   double* d_red = nullptr;    // per-CTA partial sums of cg_vector_kernel
   // multi-GPU exchange of the per-iteration partial products over NVLink peer memory (cg_kernel.cuh: xchg_push_kernel +
   // the gather in cg_vector_kernel); replaces the ncclAllReduce inside the PCG iteration when every peer could be mapped
@@ -1220,6 +1250,8 @@ int sparse_analyse(b200_handle* h) {
   OK(upload(h, sp.blk_off, &v.blk_off));
   OK(upload(h, sp.blk_ld, &v.blk_ld));
   OK(upload(h, sp.cnt, &h->d_sp_cnt_init));
+  OK(upload(h, sp.cnt_inv, &h->d_sp_cnt_inv));
+  h->sp_selinv_flops = sp.selinv_flops;
   OK(dev_alloc(h, &v.v, 9 * static_cast<size_t>(h->C)));
   OK(dev_alloc(h, &v.cnt, sp.cnt.size()));
   OK(dev_alloc(h, &v.ticket, 2));
@@ -1245,6 +1277,12 @@ int sparse_analyse(b200_handle* h) {
   h->sp_smem32 = sparse_smem_bytes<float>(sp.max_width);
   OK(grid(sparse_factor_kernel<double, true>, sparse_factor_kernel<double, false>, h->sp_smem, &h->sp_grid));
   OK(grid(sparse_factor_kernel<float, true>, sparse_factor_kernel<float, false>, h->sp_smem32, &h->sp_grid32));
+  {   // the selected inversion (b200_covariance_compute): its own cooperative grid, at most one CTA per supernode
+    h->sp_selinv_smem = selinv_smem_bytes(sp.max_width);
+    int a = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, sparse_selinv_kernel, kSpThreads, h->sp_selinv_smem));
+    h->sp_selinv_grid = a < 1 ? 0 : std::max(1, std::min(a * h->sm_count, sp.ns));   // 0: no CTA fits (refused at use)
+  }
   CU(cudaStreamSynchronize(h->stream));   // the host vectors above go out of scope
   if (getenv("B200_VERBOSE") != nullptr) {
     const int64_t* st = sp.stats;
@@ -1288,10 +1326,44 @@ void sparse_drop(b200_handle* h) {
   dev_free(h, h->spv32.L);
   dev_free(h, h->spv32.v);
   dev_free(h, h->d_sp_cnt_init);
+  dev_free(h, h->d_sp_cnt_inv);
+  dev_free(h, h->d_cov_z);   // Z's scratch has the factor's layout (the snapshot does not)
   h->spv = SparseView<double>{};
   h->spv32 = SparseView<float>{};
   h->sp_storage = 0;
   h->sp_ready = false;
+}
+
+// One cooperative launch of sparse_factor_kernel<T, kFactor> on v (counters and ticket set by the caller).
+template <typename T, bool kFactor>
+int sparse_factor_launch(b200_handle* h, SparseView<T>& v, int grid, size_t smem) {
+  cudaError_t le = cudaSuccess;
+  OK(launch(h, kFactor ? K_SPARSE_FACTOR : K_SPARSE_SOLVE, [&] {
+    void* args[] = {&v};
+    le = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(sparse_factor_kernel<T, kFactor>), dim3(grid), dim3(kSpThreads),
+                                     args, smem, h->stream);
+  }));
+  CU(le);
+  return B200_OK;
+}
+
+// S + D_f^2 scattered into v's factor storage (allocated here on first use) and factored in T, with the triangular solves of
+// the current rhs in the same launch; false in *ok when a pivot is not positive.  Shared by the solves and the covariance.
+template <typename T>
+int sparse_factor(b200_handle* h, SparseView<T>& v, int grid, size_t smem, const double* Df, bool* ok) {
+  if (v.L == nullptr) OK(dev_alloc(h, &v.L, static_cast<size_t>(h->sp_storage)));
+  CU(cudaMemsetAsync(v.L, 0, sizeof(T) * static_cast<size_t>(h->sp_storage), h->stream));
+  CU(cudaMemcpyAsync(v.cnt, h->d_sp_cnt_init, sizeof(int) * 2 * static_cast<size_t>(v.ns), cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemsetAsync(v.ticket, 0, 2 * sizeof(int), h->stream));
+  OK(launch(h, K_SPARSE_SCATTER, [&] {
+    const int g = std::max(1, std::min((h->xsv.num_blocks + 7) / 8, h->sm_count * 8));
+    sparse_scatter_kernel<T><<<g, 256, 0, h->stream>>>(v, h->xsv, Df, h->d_rhs);
+  }));
+  OK((sparse_factor_launch<T, true>(h, v, grid, smem)));
+  CU(cudaMemcpyAsync(h->h_fail, v.fail, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  *ok = h->h_fail[0] == 0;
+  return B200_OK;
 }
 
 // The factorisation of S + D_f^2 in T, its solve and the refinement's (1 + h->refine solves), into h->d_sol; false in *ok
@@ -1301,27 +1373,7 @@ int sparse_factor_solve(b200_handle* h, SparseView<T>& v, int grid, size_t smem,
   if (static_cast<double>(sizeof(T)) * static_cast<double>(h->sp_storage) > kFactorMaxBytes)
     return fail(B200_ERR_UNSUPPORTED, "sparse factor of %d cameras needs %.1f GB", h->C,
                 static_cast<double>(sizeof(T)) * static_cast<double>(h->sp_storage) / 1e9);
-  if (v.L == nullptr) OK(dev_alloc(h, &v.L, static_cast<size_t>(h->sp_storage)));
-  CU(cudaMemsetAsync(v.L, 0, sizeof(T) * static_cast<size_t>(h->sp_storage), h->stream));
-  CU(cudaMemcpyAsync(v.cnt, h->d_sp_cnt_init, sizeof(int) * 2 * static_cast<size_t>(v.ns), cudaMemcpyDeviceToDevice, h->stream));
-  CU(cudaMemsetAsync(v.ticket, 0, 2 * sizeof(int), h->stream));
-  OK(launch(h, K_SPARSE_SCATTER, [&] {
-    const int g = std::max(1, std::min((h->xsv.num_blocks + 7) / 8, h->sm_count * 8));
-    sparse_scatter_kernel<T><<<g, 256, 0, h->stream>>>(v, h->xsv, Df, h->d_rhs);
-  }));
-  auto run = [&](auto kernel, int kid) -> int {
-    cudaError_t le = cudaSuccess;
-    OK(launch(h, kid, [&] {
-      void* args[] = {&v};
-      le = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(kSpThreads), args, smem, h->stream);
-    }));
-    CU(le);
-    return B200_OK;
-  };
-  OK(run(sparse_factor_kernel<T, true>, K_SPARSE_FACTOR));
-  CU(cudaMemcpyAsync(h->h_fail, v.fail, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  *ok = h->h_fail[0] == 0;
+  OK(sparse_factor(h, v, grid, smem, Df, ok));
   if (!*ok) return B200_OK;
   OK(launch(h, K_SPARSE_SCATTER, [&] {
     sparse_gather_kernel<T><<<(9 * h->C + 255) / 256, 256, 0, h->stream>>>(v, h->d_sol);
@@ -1330,7 +1382,7 @@ int sparse_factor_solve(b200_handle* h, SparseView<T>& v, int grid, size_t smem,
     OK(refine_residual_dev(h, v.pinv, v.v));
     CU(cudaMemcpyAsync(v.cnt, h->d_sp_cnt_init, sizeof(int) * 2 * static_cast<size_t>(v.ns), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaMemsetAsync(v.ticket, 0, sizeof(int), h->stream));
-    OK(run(sparse_factor_kernel<T, false>, K_SPARSE_SOLVE));
+    OK((sparse_factor_launch<T, false>(h, v, grid, smem)));
     OK(refine_accumulate_dev(h, v.pinv, static_cast<const T*>(v.v), true));
   }
   return B200_OK;
@@ -1664,6 +1716,7 @@ int set_func_attributes(int smem_optin) {
   OK(raise_smem_limit(sparse_factor_kernel<double, false>, lim));
   OK(raise_smem_limit(sparse_factor_kernel<float, true>, lim));
   OK(raise_smem_limit(sparse_factor_kernel<float, false>, lim));
+  OK(raise_smem_limit(sparse_selinv_kernel, lim));
   return B200_OK;
 }
 
@@ -2212,6 +2265,147 @@ int minimize(Side side, Strategy strategy, const b200_lm_options* opt, double* s
 }  // namespace
 
 // ================================================================================================ C ABI
+// Covariance (b200_covariance_compute)
+namespace {
+
+// b200_covariance_compute's apply_loss_function holds for that call only: the handle's own setting comes back on every exit.
+struct ApplyLossGuard {
+  b200_handle* h;
+  bool saved;
+  ~ApplyLossGuard() { h->apply_loss = saved; }
+};
+
+// S's block pattern on the host and its block row pointers on the device, once per handle (it depends on the rows only).
+int cov_pattern(b200_handle* h) {
+  if (h->d_cov_row_ptr != nullptr) return B200_OK;
+  XsPattern xp;
+  xs_pattern(h->C, h->N, h->h_cam_idx.data(), h->h_pt_idx.data(), h->h_pt_ptr.data(), &xp);
+  h->cov_row_ptr = xp.row_ptr;
+  h->cov_blk_col = xp.blk_col;
+  OK(upload(h, h->cov_row_ptr, &h->d_cov_row_ptr));
+  CU(cudaStreamSynchronize(h->stream));
+  return B200_OK;
+}
+
+// SPARSE_SCHUR: S with D = 0 (D' = 1 on constant components) factored by sparse_factor_kernel, Z on L's pattern by
+// sparse_selinv_kernel, copied to S's blocks (h->d_cov_s).  *factored = false when a pivot is not positive.
+int cov_sparse_dev(b200_handle* h, bool* factored) {
+  if (!h->sp_ready) OK(sparse_analyse(h));
+  SparseView<double>& v = h->spv;
+  if (h->sp_selinv_grid < 1)
+    return fail(B200_ERR_UNSUPPORTED, "no CTA of the selected inversion fits an SM (%zu bytes of shared memory)", h->sp_selinv_smem);
+  OK(cov_pattern(h));
+  // what is resident at once: the FP64 factor, Z, Z on S's blocks, and a float factor a mixed-precision solve left
+  const double bytes = 16.0 * static_cast<double>(h->sp_storage) + 648.0 * static_cast<double>(h->cov_blk_col.size()) +
+                       (h->spv32.L != nullptr ? 4.0 * static_cast<double>(h->sp_storage) : 0.0);
+  if (bytes > kFactorMaxBytes) return fail(B200_ERR_UNSUPPORTED, "covariance of %d cameras needs %.1f GB of factor and inverse", h->C, bytes / 1e9);
+  if (h->d_cov_z == nullptr) OK(dev_alloc(h, &h->d_cov_z, static_cast<size_t>(h->sp_storage)));
+  if (h->d_cov_s == nullptr) OK(dev_alloc(h, &h->d_cov_s, 81 * h->cov_blk_col.size()));
+  OK(schur_init_dev(h, h->d_residuals, nullptr));   // (E'E)^-1, identity on constant points
+  OK(xs_assemble_dev(h));
+  const double* Df = h->cur_D != nullptr ? h->cur_D + 3 * static_cast<size_t>(h->P) : nullptr;
+  OK(sparse_factor(h, v, h->sp_grid, h->sp_smem, Df, factored));
+  if (!*factored) return B200_OK;
+  cudaError_t le = cudaSuccess;
+  const uint8_t* fixed_f = h->fixed_any ? h->d_fixed + 3 * static_cast<size_t>(h->P) : nullptr;
+  OK(launch(h, K_MISC, [&] {
+    selinv_pivots_kernel<<<flat_grid(h, 9 * static_cast<size_t>(h->C), 256), 256, 0, h->stream>>>(v, h->xsv, h->d_cov_row_ptr, Df,
+                                                                                                 fixed_f, h->d_cov_min);
+  }));
+  CU(cudaMemcpyAsync(v.cnt, h->d_sp_cnt_inv, sizeof(int) * static_cast<size_t>(v.ns), cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemsetAsync(v.ticket, 0, sizeof(int), h->stream));
+  OK(launch(h, K_SELINV, [&] {
+    void* args[] = {&v, &h->d_cov_z};
+    le = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(sparse_selinv_kernel), dim3(h->sp_selinv_grid), dim3(kSpThreads), args,
+                                     h->sp_selinv_smem, h->stream);
+  }));
+  CU(le);
+  const int nb = static_cast<int>(h->cov_blk_col.size());
+  return launch(h, K_SELINV, [&] {
+    selinv_blocks_kernel<<<std::max(1, std::min((nb + 7) / 8, h->sm_count * 8)), 256, 0, h->stream>>>(v, nb, h->d_cov_z, h->d_cov_s);
+  }, false);
+}
+
+// DENSE_SCHUR: the FP64 dense assembly of the solves into h->d_cov_dense, cusolverDnDpotrf, then cusolverDnDpotri: Z's lower
+// triangle.  *factored = false when potrf finds a non-positive pivot.
+int cov_dense_dev(b200_handle* h, bool* factored) {
+  const int n = 9 * h->C;
+  const size_t bytes = sizeof(double) * static_cast<size_t>(n) * n;
+  // what is resident at once: the covariance's matrix and workspace, and whatever dense solves left allocated (their FP64
+  // matrix and workspace, and the float copy of mixed precision)
+  auto resident = [&](size_t cov_work) {
+    size_t b = bytes + sizeof(double) * cov_work;
+    if (h->d_dense_s != nullptr) b += bytes + sizeof(double) * static_cast<size_t>(h->dense_lwork);
+    if (h->d_dense_s32 != nullptr) b += bytes / 2 + sizeof(float) * static_cast<size_t>(h->dense_lwork32);
+    return b;
+  };
+  const size_t cap = static_cast<size_t>(48) << 30;
+  if (resident(0) > cap)
+    return fail(B200_ERR_UNSUPPORTED, "dense covariance of %d cameras needs %.1f GB", h->C, resident(0) / 1e9);
+  if (!load_cusolver()) return fail(B200_ERR_UNSUPPORTED, "cannot load libcusolver.so.11: %s", dlerror());
+  if (!g_cusolver.potri_ok) return fail(B200_ERR_UNSUPPORTED, "the loaded cuSOLVER lacks cusolverDnDpotri (covariance)");
+  if (h->cusolver == nullptr) {
+    if (g_cusolver.Create(&h->cusolver) != 0) return fail(B200_ERR_CUDA, "cusolverDnCreate failed");
+    if (g_cusolver.SetStream(h->cusolver, h->stream) != 0) return fail(B200_ERR_CUDA, "cusolverDnSetStream failed");
+  }
+  if (h->d_cov_dense == nullptr) {
+    OK(dev_alloc(h, &h->d_cov_dense, static_cast<size_t>(n) * n));
+    OK(dev_alloc(h, &h->d_cov_diag, static_cast<size_t>(n)));
+    int a = 0, b = 0;
+    if (g_cusolver.DpotrfBufferSize(h->cusolver, /*CUBLAS_FILL_MODE_LOWER*/ 0, n, h->d_cov_dense, n, &a) != 0)
+      return fail(B200_ERR_CUDA, "cusolverDnDpotrf_bufferSize failed");
+    if (g_cusolver.DpotriBufferSize(h->cusolver, 0, n, h->d_cov_dense, n, &b) != 0)
+      return fail(B200_ERR_CUDA, "cusolverDnDpotri_bufferSize failed");
+    h->cov_lwork = std::max(1, std::max(a, b));
+    if (resident(static_cast<size_t>(h->cov_lwork)) > cap) {   // refused with nothing left half-allocated
+      dev_free(h, h->d_cov_dense);
+      dev_free(h, h->d_cov_diag);
+      return fail(B200_ERR_UNSUPPORTED, "dense covariance of %d cameras needs %.1f GB with its workspace", h->C,
+                  resident(static_cast<size_t>(h->cov_lwork)) / 1e9);
+    }
+    OK(dev_alloc(h, &h->d_cov_work, static_cast<size_t>(h->cov_lwork)));
+  }
+  OK(schur_init_dev(h, h->d_residuals, nullptr));
+  const double* Df = h->cur_D != nullptr ? h->cur_D + 3 * static_cast<size_t>(h->P) : nullptr;
+  CU(cudaMemsetAsync(h->d_cov_dense, 0, bytes, h->stream));
+  OK(launch(h, K_DIAG_BLOCKS, [&] {
+    dense_schur_assemble_kernel<<<std::max(1, std::min(h->P, h->sm_count * 8)), kDsThreads, 0, h->stream>>>(h->view, h->d_ete_inv, h->d_cov_dense, static_cast<size_t>(n));
+  }));
+  OK(launch(h, K_MISC, [&] {
+    dense_schur_diagonal_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(n, Df, h->d_cov_dense, static_cast<size_t>(n));
+    dense_diagonal_copy_kernel<<<flat_grid(h, n, 256), 256, 0, h->stream>>>(n, h->d_cov_dense, h->d_cov_diag);
+  }));
+  int* info = reinterpret_cast<int*>(h->d_cov_min + 1);
+  if (g_cusolver.Dpotrf(h->cusolver, 0, n, h->d_cov_dense, n, h->d_cov_work, h->cov_lwork, info) != 0)
+    return fail(B200_ERR_CUDA, "cusolverDnDpotrf failed");
+  CU(cudaMemcpyAsync(h->h_fail, info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  *factored = h->h_fail[0] == 0;
+  if (!*factored) return B200_OK;
+  const uint8_t* fixed_f = h->fixed_any ? h->d_fixed + 3 * static_cast<size_t>(h->P) : nullptr;
+  OK(launch(h, K_MISC, [&] {
+    dense_pivots_kernel<<<flat_grid(h, n, 256), 256, 0, h->stream>>>(n, h->d_cov_dense, h->d_cov_diag, fixed_f, h->d_cov_min);
+  }));
+  int potri = 0;
+  OK(launch(h, K_SELINV, [&] { potri = g_cusolver.Dpotri(h->cusolver, 0, n, h->d_cov_dense, n, h->d_cov_work, h->cov_lwork, info); }));
+  if (potri != 0) return fail(B200_ERR_CUDA, "cusolverDnDpotri failed");
+  return launch(h, K_SELINV, [&] {
+    dense_symmetrize_kernel<<<h->sm_count * 8, 256, 0, h->stream>>>(static_cast<long long>(n), h->d_cov_dense);
+  }, false);
+}
+
+template <bool kDense>
+ZAccess<kDense> cov_access(const b200_handle* h) {
+  ZAccess<kDense> z{};
+  z.Z = kDense ? h->d_cov_dense : h->d_cov_s;
+  z.blk_row_ptr = h->d_cov_row_ptr;
+  z.blk_col = h->xsv.blk_col;
+  z.n = 9LL * h->C;
+  return z;
+}
+
+}  // namespace
+
 extern "C" {
 
 const char* b200_last_error(void) { return g_error.c_str(); }
@@ -2272,6 +2466,31 @@ int b200_plan_sparse_schur_ordered(const b200_ba_desc* desc, int ordering_type, 
     for (int k = 0; k < C; ++k) cam_perm_out[k] = sp.perm[k];
   if (stats_out != nullptr)
     for (int k = 0; k < B200_SPARSE_STATS; ++k) stats_out[k] = sp.stats[k];
+  return B200_OK;
+}
+
+int b200_plan_sparse_selinv(const b200_ba_desc* desc, int ordering_type, int32_t* num_supernodes, int32_t* sn_first_out,
+                            int32_t* order_out, int32_t* counter_out) {
+  if (ordering_type != B200_AMD && ordering_type != B200_NESDIS)
+    return fail(B200_ERR_INVALID_ARGUMENT, "linear_solver_ordering_type must be B200_AMD or B200_NESDIS, not %d", ordering_type);
+  if (desc == nullptr || desc->cam_idx == nullptr || desc->pt_idx == nullptr || num_supernodes == nullptr)
+    return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  const int C = desc->num_cameras, P = desc->num_points;
+  const int N = static_cast<int>(desc->num_observations);
+  if (C <= 0 || P <= 0 || N <= 0) return fail(B200_ERR_INVALID_ARGUMENT, "empty problem");
+  std::vector<int> ptr;
+  OK(validate_rows(desc, &ptr));
+  XsPattern xp;
+  xs_pattern(C, N, desc->cam_idx, desc->pt_idx, ptr.data(), &xp);
+  SparsePlan sp;
+  plan_sparse_schur(C, xp.blk_row, xp.blk_col, ordering_type, &sp);
+  *num_supernodes = sp.ns;
+  for (int s = 0; s <= sp.ns; ++s)
+    if (sn_first_out != nullptr) sn_first_out[s] = sp.sn_first[s];
+  for (int s = 0; s < sp.ns; ++s) {
+    if (order_out != nullptr) order_out[s] = sp.order[s];
+    if (counter_out != nullptr) counter_out[s] = sp.cnt_inv[s];
+  }
   return B200_OK;
 }
 
@@ -3031,6 +3250,124 @@ int b200_set_linear_solver_ordering_type(b200_handle* h, int type) {
   CU(cudaSetDevice(h->device));
   sparse_drop(h);
   h->ordering = type;
+  return B200_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Covariance
+void b200_covariance_options_default(b200_covariance_options* o) {
+  o->algorithm = B200_SPARSE_SCHUR;
+  o->min_reciprocal_condition_number = 1e-14;   // covariance.h:294
+  o->apply_loss_function = 1;                   // covariance.h:339
+}
+
+int b200_covariance_compute(b200_handle* h, const double* state, const b200_covariance_options* o, int* valid) {
+  if (h == nullptr || state == nullptr || o == nullptr || valid == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  if (o->algorithm == B200_ITERATIVE_SCHUR)
+    return fail(B200_ERR_UNSUPPORTED, "covariance needs an exact factorisation: B200_SPARSE_SCHUR or B200_DENSE_SCHUR");
+  if (o->algorithm != B200_SPARSE_SCHUR && o->algorithm != B200_DENSE_SCHUR)
+    return fail(B200_ERR_INVALID_ARGUMENT, "covariance algorithm must be B200_SPARSE_SCHUR or B200_DENSE_SCHUR, not %d", o->algorithm);
+  if (!std::isfinite(o->min_reciprocal_condition_number) || o->min_reciprocal_condition_number < 0.0)
+    return fail(B200_ERR_INVALID_ARGUMENT, "min_reciprocal_condition_number %g", o->min_reciprocal_condition_number);
+  if (h->world > 1) return fail(B200_ERR_UNSUPPORTED, "covariance needs the explicit Schur complement, which is single-GPU");
+  *valid = 0;
+  CU(cudaSetDevice(h->device));
+  h->cov_valid = false;   // a new compute replaces the snapshot, also when it fails
+  ApplyLossGuard guard{h, h->apply_loss};
+  h->apply_loss = o->apply_loss_function != 0;
+  OK(up_params(h, h->d_state, state));
+  h->residuals_resident = false;
+  double cost = 0.0;
+  OK(evaluate_dev(h, h->d_state, h->d_residuals, nullptr, true, nullptr, &cost));
+  h->residuals_resident = true;
+  if (h->d_cov_min == nullptr) OK(dev_alloc(h, &h->d_cov_min, 2));
+  if (h->d_cov_pts == nullptr) OK(dev_alloc(h, &h->d_cov_pts, 9 * static_cast<size_t>(h->P)));
+  const double inf = std::numeric_limits<double>::infinity();
+  CU(cudaMemcpyAsync(h->d_cov_min, &inf, sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  const bool dense = o->algorithm == B200_DENSE_SCHUR;
+  bool factored = false;
+  int rc = dense ? cov_dense_dev(h, &factored) : cov_sparse_dev(h, &factored);
+  // the Schur initialisation, S and the factor now hold the covariance's: the next solve rebuilds them
+  h->schur_ready = false;
+  h->xs_ready = false;
+  h->xs_diag_ready = false;
+  h->q_from_init = false;
+  OK(rc);
+  if (!factored) {
+    if (getenv("B200_VERBOSE") != nullptr) fprintf(stderr, "[b200ba] covariance: S is not positive definite\n");
+    return B200_OK;
+  }
+  const int* perm = h->permuted ? h->d_pt_perm : nullptr;
+  OK(launch(h, K_COV_POINTS, [&] {
+    const int g = std::max(1, std::min((h->P + 7) / 8, h->sm_count * 16));
+    if (dense) covariance_point_kernel<true><<<g, 256, 0, h->stream>>>(h->view, cov_access<true>(h), h->d_fixed, perm, h->d_cov_pts, h->d_cov_min);
+    else covariance_point_kernel<false><<<g, 256, 0, h->stream>>>(h->view, cov_access<false>(h), h->d_fixed, perm, h->d_cov_pts, h->d_cov_min);
+  }));
+  unsigned long long bits = 0;
+  CU(cudaMemcpyAsync(&bits, h->d_cov_min, sizeof(bits), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  double rcond = 0.0;
+  std::memcpy(&rcond, &bits, sizeof(rcond));
+  if (getenv("B200_VERBOSE") != nullptr)
+    fprintf(stderr, "[b200ba] covariance: %s, selected inversion %.3g flops, min pivot / diagonal %.3e (threshold %.3e)\n",
+            dense ? "dense potri" : "sparse", dense ? 0.0 : h->sp_selinv_flops, rcond, o->min_reciprocal_condition_number);
+  if (!(rcond >= o->min_reciprocal_condition_number)) return B200_OK;
+  h->cov_alg = o->algorithm;
+  h->cov_cam_fixed.assign(static_cast<size_t>(h->C), 0);
+  if (h->fixed_any)
+    for (int c = 0; c < h->C; ++c) h->cov_cam_fixed[c] = h->h_fixed[3 * static_cast<size_t>(h->P) + 9 * static_cast<size_t>(c)];
+  h->cov_valid = true;
+  *valid = 1;
+  return B200_OK;
+}
+
+int b200_covariance_cameras(b200_handle* h, int num_pairs, const int32_t* pairs, double* out) {
+  if (h == nullptr || num_pairs < 0 || (num_pairs > 0 && (pairs == nullptr || out == nullptr)))
+    return fail(B200_ERR_INVALID_ARGUMENT, "null argument or num_pairs < 0");
+  if (!h->cov_valid) return fail(B200_ERR_INVALID_ARGUMENT, "no valid covariance: b200_covariance_compute first (CHECK(is_valid_))");
+  const bool dense = h->cov_alg == B200_DENSE_SCHUR;
+  std::vector<int4> desc(static_cast<size_t>(num_pairs));
+  for (int q = 0; q < num_pairs; ++q) {
+    const int i = pairs[2 * q], j = pairs[2 * q + 1];
+    if (i < 0 || i >= h->C || j < 0 || j >= h->C)
+      return fail(B200_ERR_INVALID_ARGUMENT, "pair %d: cameras (%d, %d) outside [0, %d)", q, i, j, h->C);
+    int b = -1;
+    if (!dense) {
+      const int a = std::min(i, j), c = std::max(i, j);
+      auto first = h->cov_blk_col.begin() + h->cov_row_ptr[a], last = h->cov_blk_col.begin() + h->cov_row_ptr[a + 1];
+      auto it = std::lower_bound(first, last, c);
+      if (it == last || *it != c)
+        return fail(B200_ERR_INVALID_ARGUMENT, "pair %d: cameras (%d, %d) share no point, so SPARSE_SCHUR does not compute their block "
+                    "(DENSE_SCHUR does)", q, i, j);
+      b = static_cast<int>(it - h->cov_blk_col.begin());
+    }
+    desc[q] = make_int4(i, j, b, h->cov_cam_fixed[i] != 0 || h->cov_cam_fixed[j] != 0);
+  }
+  if (num_pairs == 0) return B200_OK;
+  CU(cudaSetDevice(h->device));
+  if (h->cov_pairs_cap < desc.size()) {
+    dev_free(h, h->d_cov_pairs);
+    dev_free(h, h->d_cov_out);
+    OK(dev_alloc(h, &h->d_cov_pairs, desc.size()));
+    OK(dev_alloc(h, &h->d_cov_out, 81 * desc.size()));
+    h->cov_pairs_cap = desc.size();
+  }
+  CU(cudaMemcpyAsync(h->d_cov_pairs, desc.data(), sizeof(int4) * desc.size(), cudaMemcpyHostToDevice, h->stream));
+  OK(launch(h, K_COV_GATHER, [&] {
+    const int g = flat_grid(h, 81 * desc.size(), 256);
+    if (dense) covariance_gather_kernel<true><<<g, 256, 0, h->stream>>>(cov_access<true>(h), num_pairs, h->d_cov_pairs, h->d_cov_out);
+    else covariance_gather_kernel<false><<<g, 256, 0, h->stream>>>(cov_access<false>(h), num_pairs, h->d_cov_pairs, h->d_cov_out);
+  }));
+  CU(cudaMemcpyAsync(out, h->d_cov_out, sizeof(double) * 81 * desc.size(), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  return B200_OK;
+}
+
+int b200_covariance_points(b200_handle* h, double* out) {
+  if (h == nullptr || out == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+  if (!h->cov_valid) return fail(B200_ERR_INVALID_ARGUMENT, "no valid covariance: b200_covariance_compute first (CHECK(is_valid_))");
+  CU(cudaSetDevice(h->device));
+  CU(cudaMemcpyAsync(out, h->d_cov_pts, sizeof(double) * 9 * static_cast<size_t>(h->P), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
   return B200_OK;
 }
 

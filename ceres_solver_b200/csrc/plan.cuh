@@ -63,6 +63,9 @@ enum KernelId {
   K_DOGLEG_GN,
   K_DOGLEG_STEP,
   K_REFINE,
+  K_SELINV,
+  K_COV_POINTS,
+  K_COV_GATHER,
   K_MISC,
   K_COUNT
 };
@@ -71,7 +74,8 @@ const char* const kKernelNames[K_COUNT] = {"evaluate_jacobian", "evaluate_cost",
                                            "schur_multiply", "schur_multiply_big_points", "camera_reduce", "schur_diag_blocks", "invert_9x9", "back_substitute",
                                            "model_cost", "cg_vector", "lm_vector", "pmv_right_e", "pmv_right_f", "pmv_left_e", "pmv_left_f", "schur_pcg",
                                            "sparse_scatter", "sparse_factor", "sparse_solve", "dogleg_gram", "dogleg_diagonal", "dogleg_gn", "dogleg_step",
-                                           "refine_convert", "misc"};
+                                           "refine_convert", "selected_inversion", "covariance_points",
+                                           "covariance_gather", "misc"};
 
 // Development switches (A/B measurements of kernel variants and tuning knobs) exist only in builds with
 // -DB200_DEV_KNOBS; the product library has a single code path per problem class and reads no such variable.

@@ -549,6 +549,9 @@ struct SparsePlan {
   std::vector<int4> upd;                    // {d, k0, k1, 0}: rows k0..k1-1 of descendant d lie in this supernode's columns
   std::vector<int> ntf_ptr, ntf;            // [ns + 1] / the supernodes each supernode updates, ascending
   std::vector<int> cnt;                     // [2 ns] initial dependency counters of the forward and backward tasks
+  std::vector<int> cnt_inv;                 // [ns] ... of the selected-inversion tasks (covariance.cuh): the supernodes
+                                            // each supernode updates, 0 for a root
+  double selinv_flops = 0.0;                // flops of the selected inversion (covariance.cuh) on this factor
   std::vector<long long> blk_off;           // per S block: offset of its 9x9 block in the factor storage
   std::vector<int> blk_ld;                  // ... and the panel's leading dimension, negated when the block goes in transposed
   int max_width = 0;                        // widest supernode (scalar columns)
@@ -659,6 +662,16 @@ inline void plan_sparse_schur(int C, const std::vector<int>& blk_row, const std:
     sp.cnt[s] = sp.upd_ptr[s + 1] - sp.upd_ptr[s];
     const int n = sp.ntf_ptr[s + 1] - sp.ntf_ptr[s];
     sp.cnt[ns + s] = n > 0 ? n : 1;
+  }
+  // the selected inversion has no forward tasks: a root starts at once
+  sp.cnt_inv.assign(static_cast<size_t>(ns), 0);
+  for (int s = 0; s < ns; ++s) sp.cnt_inv[s] = sp.ntf_ptr[s + 1] - sp.ntf_ptr[s];
+  // its flops per supernode of W columns and n rows below: L_ss^-1 and L_ss^-T L_ss^-1 (W^3 / 3 each), U = L_Rs L_ss^-1
+  // (n W^2), Z_Rs = -Z_RR U (2 n^2 W) and U' Z_Rs (2 n W^2)
+  sp.selinv_flops = 0.0;
+  for (int s = 0; s < ns; ++s) {
+    const double W = 9.0 * (sp.sn_first[s + 1] - sp.sn_first[s]), n = 9.0 * (sp.row_ptr[s + 1] - sp.row_ptr[s]) - W;
+    sp.selinv_flops += 2.0 * W * W * W / 3.0 + n * W * W + 2.0 * n * n * W + 2.0 * n * W * W;
   }
   // the supernodal tree (the parent of s owns the elimination-tree parent of s's last column; every descendant has a smaller
   // index), its critical paths from a leaf to a root, in supernodes and in the flops of the columns (those of the `flops`

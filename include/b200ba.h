@@ -291,6 +291,47 @@ int b200_schur_back_substitute(b200_handle* h, const double* z, double* y);     
 int b200_schur_jacobi_update(b200_handle* h, double* blocks, double* inverse);  /* each [81C], may be NULL */
 int b200_block_jacobi_update(b200_handle* h, double* inverse);                  /* JACOBI: (F'F + D_f^2)^-1 blocks, [81C] */
 
+/* ---- Covariance::Compute / GetCovarianceBlock (include/ceres/covariance.h, internal/ceres/covariance_impl.cc) for the
+ * camera blocks and the point blocks, in the Schur form: Cov(cameras) = Z = S^-1, with S the reduced camera system at D = 0
+ * (D' = 1 on constant components, as every solve uses), and Cov(p, p) = V_p^-1 + V_p^-1 (sum over rows r, s of p of
+ * W_r Z_{c_r c_s} W_s') V_p^-1, V_p = E_p'E_p, W_r = E_r'F_r.  Always FP64, single GPU.
+ * b200_covariance_compute evaluates J at `state` (as b200_evaluate with want_jacobian and residuals does: the stored J
+ * and the resident residuals are those of `state` afterwards), forms S, factors it and keeps Z and every point block on
+ * the device as a snapshot that later evaluations, solves, setters and LM runs do not change; a new compute replaces it.
+ * apply_loss_function applies to this call only: the handle's own setting comes back on every exit.  The Schur
+ * initialisation, the explicit S and the factor are left as the covariance's, so the next solve rebuilds them; the sparse
+ * analysis is reused (the handle's linear_solver_ordering_type), and use_mixed_precision_solves and the refinement count
+ * do not apply.
+ *   B200_SPARSE_SCHUR: the supernodal factor and its selected inverse, Z on the pattern of L; serves every pair (i, i) and
+ *                      every pair of cameras that share a point.
+ *   B200_DENSE_SCHUR:  cuSOLVER potrf + potri on the dense S (cusolverDnDpotri needed); serves any pair.
+ * *valid, as Covariance::Compute's bool: 0 when S or a variable point's E'E is not positive definite, or when the
+ * smallest ratio d_k / A_kk over the variable components (d_k the k-th squared pivot, A_kk the diagonal of the matrix
+ * factored), over S's factor and every point's 3x3 Cholesky, is below min_reciprocal_condition_number.  The return code
+ * stays B200_OK then.  B200_ERR_UNSUPPORTED: B200_ITERATIVE_SCHUR, a sharded handle, or storage over the caps of the
+ * solves (the sparse one counts the factor and Z).  B200_ERR_EVALUATION_FAILED: the evaluation at `state` failed. */
+typedef struct b200_covariance_options { /* Covariance::Options, include/ceres/covariance.h:240-340 */
+  int32_t algorithm;                       /* B200_SPARSE_SCHUR (default) or B200_DENSE_SCHUR */
+  double min_reciprocal_condition_number;  /* 1e-14, covariance.h:294 */
+  int32_t apply_loss_function;             /* 1, covariance.h:339 */
+} b200_covariance_options;
+void b200_covariance_options_default(b200_covariance_options* o);
+int b200_covariance_compute(b200_handle* h, const double* state, const b200_covariance_options* o, int* valid);
+/* The getters refuse with B200_ERR_INVALID_ARGUMENT before any compute and after one that set valid = 0
+ * (covariance_impl.cc:137-141).  Output is row-major 9 x 9 / 3 x 3 blocks in the caller's camera and point order, as
+ * GetCovarianceBlock writes them.  pairs[2 num_pairs]: Cov(c_i, c_j) of pair (i, j) in out[81 q..]; (j, i) returns its
+ * transpose.  A pair with a constant camera and a constant point return exact zeros (covariance_impl.cc:143-165).  A pair
+ * out of range, or (sparse) a pair of distinct cameras that share no point, is refused with nothing written. */
+int b200_covariance_cameras(b200_handle* h, int num_pairs, const int32_t* pairs, double* out);
+int b200_covariance_points(b200_handle* h, double* out); /* [9P] */
+/* The selected inversion's task graph of the analysis b200_plan_sparse_schur_ordered describes, host-only:
+ * *num_supernodes = ns; sn_first_out [ns + 1] (first position of each supernode), order_out [ns] (the factor's ticket
+ * order; the selected inversion takes it in reverse) and counter_out [ns] (the initial counter of each supernode's
+ * selected-inversion task: the number of supernodes owning one of its rows below, 0 for a root).  Buffers of C + 1 / C
+ * entries always suffice; any may be NULL. */
+int b200_plan_sparse_selinv(const b200_ba_desc* desc, int ordering_type, int32_t* num_supernodes, int32_t* sn_first_out,
+                            int32_t* order_out, int32_t* counter_out);
+
 /* ---- Device-resident trust-region loop (SURVEY §8f.3: TrustRegionMinimizer::Minimize with
  * LevenbergMarquardtStrategy, trust_region_minimizer.cc:68-137 / levenberg_marquardt_strategy.cc:69-171, or with
  * DoglegStrategy, dogleg_strategy.cc:54-717).
