@@ -7,4 +7,5 @@ from .binding import (B200Error, Problem, lib, nccl_unique_id, plan_point_order,
                       PRECOND_IDENTITY, PRECOND_JACOBI, PRECOND_SCHUR_JACOBI, PRECOND_SCHUR_POWER_SERIES_EXPANSION, ITERATIVE_SCHUR, DENSE_SCHUR,
                       SPARSE_SCHUR, SPARSE_STATS, LEVENBERG_MARQUARDT, DOGLEG, TRADITIONAL_DOGLEG, SUBSPACE_DOGLEG, AMD, NESDIS, LOSS_TRIVIAL, LOSS_HUBER,
                       LOSS_SOFT_L_ONE, LOSS_CAUCHY, LOSS_ARCTAN, LOSS_TOLERANT, LOSS_TUKEY, Loss, CovarianceOptions, plan_sparse_selinv,
+                      subset_manifold_masks,
                       LS_SUCCESS, LS_NO_CONVERGENCE, LS_FAILURE, LS_FATAL_ERROR)

@@ -98,7 +98,7 @@ class KernelStat(C.Structure):
 # Every symbol include/b200ba.h declares (tests/test_abi.py checks the library exports all of them).
 SYMBOLS = [
     "b200_plan_point_order", "b200_plan_sparse_schur", "b200_plan_sparse_schur_ordered", "b200_sparse_schur_solve", "b200_nccl_unique_id", "b200_create", "b200_destroy", "b200_last_error", "b200_num_parameters",
-    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_set_loss_functions", "b200_set_constant_blocks", "b200_plus", "b200_jacobian_squared_column_norm",
+    "b200_num_residuals", "b200_evaluate", "b200_set_apply_loss_function", "b200_set_loss_functions", "b200_set_constant_blocks", "b200_set_subset_manifolds", "b200_plus", "b200_jacobian_squared_column_norm",
     "b200_jacobian_scale_columns", "b200_jacobian_right_multiply", "b200_jacobian_left_multiply", "b200_model_cost_change",
     "b200_jacobian_get_values", "b200_jacobian_set_values", "b200_partitioned_multiply", "b200_jtj_multiply", "b200_solver_options_default",
     "b200_schur_solve", "b200_dense_schur_solve", "b200_set_exact_solve_options",
@@ -186,6 +186,23 @@ def plan_sparse_selinv(num_cameras, num_points, cam_idx, pt_idx, ordering_type=A
                                          order.ctypes.data_as(_ip), cnt.ctypes.data_as(_ip)))
     n = ns.value
     return first[:n + 1].copy(), order[:n].copy(), cnt[:n].copy()
+
+
+def subset_manifold_masks(num_cameras, num_points, camera_constant=None, point_constant=None):
+    """The bit masks b200_set_subset_manifolds takes, from boolean arrays of shape (C, 9) and (P, 3) (True = coordinate
+    held constant: SubsetManifold(9 | 3, {k : True})), or None for no SubsetManifold on any block of that kind.  Returns
+    (uint16 [C] or None, uint8 [P] or None); ValueError on a shape mismatch."""
+    out = []
+    for a, n, width, dtype, what in ((camera_constant, num_cameras, 9, np.uint16, "camera_constant"),
+                                     (point_constant, num_points, 3, np.uint8, "point_constant")):
+        if a is None:
+            out.append(None)
+            continue
+        a = np.asarray(a).astype(bool)
+        if a.shape != (int(n), width):
+            raise ValueError("%s has shape %s for (%d, %d)" % (what, a.shape, int(n), width))
+        out.append(np.ascontiguousarray((a.astype(np.uint32) << np.arange(width, dtype=np.uint32)).sum(axis=1).astype(dtype)))
+    return out[0], out[1]
 
 
 def nccl_unique_id():
@@ -278,6 +295,14 @@ class Problem:
             flags.append(a)
         _check(lib().b200_set_constant_blocks(self.h, *(None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
                                                        for a in flags)))
+
+    def set_subset_manifolds(self, camera_constant=None, point_constant=None):
+        """b200_set_subset_manifolds: boolean arrays of shape (C, 9) and (this problem's P, 3), True on the coordinates
+        each block's SubsetManifold holds constant; None = no SubsetManifold on any block of that kind.  Replaces the
+        problem's masks (Problem::SetManifold) and leaves its constant blocks alone."""
+        cam, pts = subset_manifold_masks(self.C, self.P, camera_constant, point_constant)
+        _check(lib().b200_set_subset_manifolds(self.h, None if cam is None else cam.ctypes.data_as(C.POINTER(C.c_uint16)),
+                                               None if pts is None else pts.ctypes.data_as(C.POINTER(C.c_uint8))))
 
     # ---- Jacobian as a SparseMatrix
     def squared_column_norm(self):

@@ -329,7 +329,10 @@ __global__ void __launch_bounds__(256) dense_symmetrize_kernel(long long n, doub
 }
 
 // Cov(p, p) of every point, one warp per point, into out [9P] in the caller's point order (row-major 3 x 3), zero for a
-// constant point; the pivots of each variable point's Cholesky of V_p = E_p'E_p go to the conditioning test.  Lane q takes
+// constant point; the pivots of each variable point's Cholesky of V_p = E_p'E_p go to the conditioning test.  A coordinate
+// held by a SubsetManifold (fixed == kComponentMasked) has a zero E column: V_p takes D' = 1 there, the coordinate stays
+// out of the conditioning test, and its row and column of the block are written as 0 (GetCovarianceBlock lifts the
+// tangent covariance with the 0/1 plus Jacobian).  Lane q takes
 // the row pairs q, q + 32, ... in a fixed order and the warp sums with a fixed butterfly: no atomics on values.
 template <bool kDense>
 __global__ void __launch_bounds__(256) covariance_point_kernel(ProblemView p, ZAccess<kDense> z, const uint8_t* __restrict__ fixed,
@@ -341,10 +344,11 @@ __global__ void __launch_bounds__(256) covariance_point_kernel(ProblemView p, ZA
   const double* __restrict__ F = p.F();
   for (int k = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5); k < p.P; k += nw) {
     double* o = out + 9LL * (pt_perm != nullptr ? pt_perm[k] : k);
-    if (fixed != nullptr && fixed[3LL * k] != 0) {
+    if (fixed != nullptr && fixed[3LL * k] == kComponentConstant) {
       if (lane < 9) o[lane] = 0.0;
       continue;
     }
+    const unsigned m = fixed == nullptr ? 0u : (fixed[3LL * k] != 0) | (fixed[3LL * k + 1] != 0) << 1 | (fixed[3LL * k + 2] != 0) << 2;
     const int r0 = p.pt_ptr[k], d = p.pt_ptr[k + 1] - r0;
     // V = sum_r E_r'E_r (upper triangle: 00 01 02 11 12 22)
     double v[6] = {0, 0, 0, 0, 0, 0};
@@ -404,11 +408,16 @@ __global__ void __launch_bounds__(256) covariance_point_kernel(ProblemView p, ZA
       for (int m = 0; m < 9; ++m) g[m] += __shfl_xor_sync(0xffffffffu, g[m], off);
     }
     if (lane == 0) {
+      if (m & 1u) v[0] = 1.0;   // D' = 1 on masked coordinates (their off-diagonal entries are already 0)
+      if (m & 2u) v[3] = 1.0;
+      if (m & 4u) v[5] = 1.0;
       // Cholesky of V, its pivots against V's diagonal, V^-1 = L^-T L^-1
       const double l00 = sqrt(v[0]), l10 = v[1] / l00, l20 = v[2] / l00;
       const double d1 = v[3] - l10 * l10, l11 = sqrt(d1), l21 = (v[4] - l20 * l10) / l11;
       const double d2 = v[5] - l20 * l20 - l21 * l21, l22 = sqrt(d2);
-      offer_min(min_slot, fmin(fmin(v[0] / v[0], d1 / v[3]), d2 / v[5]));   // NaN (v[0] = 0) counts as 0
+      // NaN (v[0] = 0) counts as 0; a masked coordinate offers NaN, which fmin drops
+      const double nan = __longlong_as_double(0x7ff8000000000000LL);
+      offer_min(min_slot, fmin(fmin((m & 1u) ? nan : v[0] / v[0], (m & 2u) ? nan : d1 / v[3]), (m & 4u) ? nan : d2 / v[5]));
       const double m00 = 1.0 / l00, m11 = 1.0 / l11, m22 = 1.0 / l22;   // M = L^-1 (lower)
       const double m10 = -l10 * m00 * m11, m21 = -l21 * m11 * m22;
       const double m20 = -(l20 * m00 + l21 * m10) * m22;
@@ -428,12 +437,14 @@ __global__ void __launch_bounds__(256) covariance_point_kernel(ProblemView p, ZA
       for (int a = 0; a < 3; ++a)
 #pragma unroll
         for (int b = 0; b < 3; ++b)
-          o[3 * a + b] = vi[3 * a + b] + h[3 * a] * vi[b] + h[3 * a + 1] * vi[3 + b] + h[3 * a + 2] * vi[6 + b];
+          o[3 * a + b] = ((m >> a) | (m >> b)) & 1u ? 0.0
+                                                     : vi[3 * a + b] + h[3 * a] * vi[b] + h[3 * a + 1] * vi[3 + b] + h[3 * a + 2] * vi[6 + b];
     }
   }
 }
 
-// The requested camera blocks: out [81 x n] row-major, pair q = {i, j, -, 1 = zero}.
+// The requested camera blocks: out [81 x n] row-major, pair q = {i, j, -, zero mask}: bit u (u < 9) zeroes row u, bit
+// 9 + v column v (the constant coordinates of camera i and of camera j; all of them for a constant camera).
 template <bool kDense>
 __global__ void __launch_bounds__(256) covariance_gather_kernel(ZAccess<kDense> z, int n, const int4* __restrict__ pairs,
                                                                double* __restrict__ out) {
@@ -443,7 +454,7 @@ __global__ void __launch_bounds__(256) covariance_gather_kernel(ZAccess<kDense> 
     const int4 pr = pairs[q];
     long long su, sv;
     const double* zb = z.block(pr.x, pr.y, &su, &sv);
-    out[e] = pr.w != 0 ? 0.0 : zb[u * su + v * sv];
+    out[e] = ((pr.w >> u) | (pr.w >> (9 + v))) & 1 ? 0.0 : zb[u * su + v * sv];
   }
 }
 

@@ -133,15 +133,39 @@ __device__ __forceinline__ void snavely(const double* __restrict__ cam, double X
   }
 }
 
-// Zeroes a row's cells of its constant blocks: jp when the point (component po) is constant, jc when the camera (pc) is.
-__device__ __forceinline__ void fixed_cells(const uint8_t* __restrict__ fixed, size_t po, size_t pc, double* jc, double* jp) {
-  if (__ldg(fixed + po) != 0) {
+// The packed state of one block, as the evaluate kernels read it (b200_set_constant_blocks, b200_set_subset_manifolds):
+// kBlockConstant for a constant block (a full SubsetManifold included), else bit k = coordinate k held by a SubsetManifold.
+constexpr uint16_t kBlockConstant = 0x8000;
+
+// Zeroes a row's cells of its constant blocks (mp: the point's state, mc: the camera's), before the finiteness check:
+// Ceres evaluates a constant block with jacobians[i] == nullptr, so nothing there is checked.
+__device__ __forceinline__ void constant_cells(uint32_t mp, uint32_t mc, double* jc, double* jp) {
+  if (mp & kBlockConstant) {
 #pragma unroll
     for (int k = 0; k < 6; ++k) jp[k] = 0.0;
   }
-  if (__ldg(fixed + pc) != 0) {
+  if (mc & kBlockConstant) {
 #pragma unroll
     for (int k = 0; k < 18; ++k) jc[k] = 0.0;
+  }
+}
+
+// Zeroes a row's columns of coordinates held by a SubsetManifold, after the finiteness check: Ceres checks the ambient
+// Jacobian before it multiplies by the 0/1 PlusJacobian (residual_block.cc:85-159).  The Corrector is linear per column,
+// so zeroing before it is the same as after.
+__device__ __forceinline__ void masked_cells(uint32_t mp, uint32_t mc, double* jc, double* jp) {
+  if (((mp | mc) & 0x1ffu) == 0) return;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const bool m = (mp >> k) & 1u;
+    jp[k] = m ? 0.0 : jp[k];
+    jp[3 + k] = m ? 0.0 : jp[3 + k];
+  }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    const bool m = (mc >> k) & 1u;
+    jc[k] = m ? 0.0 : jc[k];
+    jc[9 + k] = m ? 0.0 : jc[9 + k];
   }
 }
 
@@ -153,15 +177,16 @@ struct EvalArgs {
   const double* scale;   // null or [3P+9C]: Jacobi scaling fused into the Jacobian write (J <- J diag(scale))
   int* fail_flag;        // set to 1 on a non-finite residual/Jacobian entry
   LossArgs loss;
-  const uint8_t* fixed;  // [3P+9C], read with kFixed only: nonzero on the components of constant blocks
+  const uint16_t* block_state;  // [P + C] points then cameras, read with kFixed only: the packed states (kBlockConstant)
 };
 
 // kStoreJ = false (gradient without the Jacobian): J is computed, checked and used for the gradient, but the stored
 // Jacobian is left as it is.  A template parameter, so that the instantiation the LM loop runs is the same code.
 // kLoss: the class of the handle's loss set (loss.cuh).
-// kFixed: the handle holds blocks constant.  Their cells are set to 0 before anything reads them: they are not checked
-// for finiteness, not corrected by the loss, and stored, summed into the gradient and scaled as 0 (the columns
-// Program::RemoveFixedBlocks leaves out of the reduced program).
+// kFixed: the handle holds blocks or coordinates constant.  A constant block's cells are set to 0 before anything reads
+// them: they are not checked for finiteness, not corrected by the loss, and stored, summed into the gradient and scaled
+// as 0 (the columns Program::RemoveFixedBlocks leaves out of the reduced program).  A coordinate held by a SubsetManifold
+// is checked first and then set to 0 (the column its PlusJacobian drops).
 template <int kLoss, bool kWantJ, bool kStoreJ = kWantJ, bool kFixed = false>
 __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -184,7 +209,12 @@ __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs
       const double* cp = a.state + 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(cam);
       const double2 o = *reinterpret_cast<const double2*>(p.obs + 2 * row);
       snavely<kWantJ>(cp, X[0], X[1], X[2], o.x, o.y, r0, r1, jc, jp);
-      if (kFixed && kWantJ) fixed_cells(a.fixed, 3 * static_cast<size_t>(d.pt_begin + lpt), 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(cam), jc, jp);
+      uint32_t mp = 0, mc = 0;
+      if (kFixed && kWantJ) {
+        mp = __ldg(a.block_state + d.pt_begin + lpt);
+        mc = __ldg(a.block_state + p.P + cam);
+        constant_cells(mp, mc, jc, jp);
+      }
       bool finite = isfinite(r0) && isfinite(r1);
       if (kWantJ) {
 #pragma unroll
@@ -193,6 +223,7 @@ __global__ void __launch_bounds__(kTile) evaluate_kernel(ProblemView p, EvalArgs
         for (int k = 0; k < 6; ++k) finite = finite && isfinite(jp[k]);
       }
       if (!finite) atomicExch(a.fail_flag, 1);
+      if (kFixed && kWantJ) masked_cells(mp, mc, jc, jp);
       cost = apply_loss<kLoss, kWantJ>(row_loss_entry<kLoss>(a.loss, row), r0, r1, jc, jp);
       if (a.residuals != nullptr) *reinterpret_cast<double2*>(a.residuals + 2 * row) = make_double2(r0, r1);
       if (kWantJ) {
@@ -320,20 +351,27 @@ __global__ void __launch_bounds__(kTile) sqnorm_kernel(ProblemView p, double* ou
   }
 }
 
-// Zeroes the stored cells of constant blocks (fixed: [3P+9C], nonzero on their components): the E cells of rows whose point
-// is constant, the F cells of rows whose camera is.  Same flat walk as scale_kernel.
+// Zeroes the stored cells of constant components (fixed: [3P+9C], nonzero on the components of constant blocks and on
+// coordinates held by a SubsetManifold), column by column.  Same flat walk as scale_kernel: E cell [2][3] as 3 double2,
+// element e -> column e % 3; F cell [2][9] as 9 double2, element e -> column e % 9.
 __global__ void __launch_bounds__(256) fixed_mask_kernel(ProblemView p, const uint8_t* __restrict__ fixed) {
   const size_t nE2 = 3 * static_cast<size_t>(p.N), nF2 = 9 * static_cast<size_t>(p.N);
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   double2* E2 = reinterpret_cast<double2*>(p.E());
   double2* F2 = reinterpret_cast<double2*>(p.F());
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nE2 + nF2; i += stride) {
-    if (i < nE2) {
-      if (fixed[3 * static_cast<size_t>(p.pt_of_row[i / 3])] != 0) E2[i] = make_double2(0.0, 0.0);
-    } else {
-      const size_t j = i - nE2;
-      if (fixed[3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(p.cam_idx[j / 9])] != 0) F2[j] = make_double2(0.0, 0.0);
-    }
+    const bool e_cell = i < nE2;
+    const size_t j = e_cell ? i : i - nE2;
+    const int w = e_cell ? 3 : 9, el = 2 * static_cast<int>(j % w);
+    const uint8_t* f = e_cell ? fixed + 3 * static_cast<size_t>(p.pt_of_row[j / 3])
+                              : fixed + 3 * static_cast<size_t>(p.P) + 9 * static_cast<size_t>(p.cam_idx[j / 9]);
+    const bool zx = f[el % w] != 0, zy = f[(el + 1) % w] != 0;
+    if (!zx && !zy) continue;
+    double2* c = e_cell ? E2 + j : F2 + j;
+    double2 v = *c;
+    if (zx) v.x = 0.0;
+    if (zy) v.y = 0.0;
+    *c = v;
   }
 }
 

@@ -94,7 +94,7 @@ struct EvalV2Args {
   const double* scale;   // null or [3P+9C]
   int* fail_flag;
   LossArgs loss;
-  const uint8_t* fixed;  // [3P+9C], kFixed only (evaluate_kernel)
+  const uint16_t* block_state;  // [P + C], kFixed only (evaluate_kernel)
 };
 
 constexpr int kEvalScratch = 3;  // doubles per lane in the exchange scratch
@@ -103,7 +103,7 @@ __host__ __device__ inline int eval_v2_per_warp_bytes() { return 32 * 144 + 32 *
 // Evaluate residuals, Jacobian (written through a per-warp staging buffer + TMA bulk store), cost, gradient and the
 // squared column norms of the Jacobian as written (i.e. after the fused Jacobi scaling).
 // kStoreJ = false (gradient without the Jacobian): as evaluate_kernel<kLoss, true, false>, the Jacobian is left as it is.
-// kFixed: constant blocks' cells are 0, as in evaluate_kernel.
+// kFixed: constant blocks' cells and coordinates held by a SubsetManifold are 0, as in evaluate_kernel.
 template <int kLoss, bool kStoreJ, bool kFixed = false>
 __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v, EvalV2Args a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -144,13 +144,19 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
       const double* cp = a.state + camoff + 9 * static_cast<size_t>(cam);
       const double2 o = *reinterpret_cast<const double2*>(v.p.obs + 2 * row);
       snavely<true>(cp, a.state[po], a.state[po + 1], a.state[po + 2], o.x, o.y, r0, r1, jc, jp);
-      if (kFixed) fixed_cells(a.fixed, po, camoff + 9 * static_cast<size_t>(cam), jc, jp);
+      uint32_t mp = 0, mc = 0;
+      if (kFixed) {
+        mp = __ldg(a.block_state + wt.pt_begin + sg.lpt);
+        mc = __ldg(a.block_state + v.p.P + cam);
+        constant_cells(mp, mc, jc, jp);
+      }
       bool finite = isfinite(r0) && isfinite(r1);
 #pragma unroll
       for (int k = 0; k < 18; ++k) finite = finite && isfinite(jc[k]);
 #pragma unroll
       for (int k = 0; k < 6; ++k) finite = finite && isfinite(jp[k]);
       if (!finite) atomicExch(a.fail_flag, 1);
+      if (kFixed) masked_cells(mp, mc, jc, jp);
       cost += apply_loss<kLoss, true>(row_loss_entry<kLoss>(a.loss, row), r0, r1, jc, jp);
       if (a.residuals != nullptr) *reinterpret_cast<double2*>(a.residuals + 2 * row) = make_double2(r0, r1);
     }

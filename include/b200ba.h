@@ -190,9 +190,34 @@ int b200_set_loss_functions(b200_handle* h, const b200_loss* losses, int num_los
  *    them after every upload; cells of blocks made variable keep what they held until the next evaluation with J.  The
  *    explicit S, the Schur initialisation and the preconditioner are invalidated; the resident residuals are kept.
  *  - Sharded handles: each rank passes its own points' flags and the same camera flags.
- * B200_ERR_INVALID_ARGUMENT, with the handle unchanged: h == NULL, or a row whose camera and point are both constant
- * (Ceres moves such a row's cost into fixed_cost; drop the row from the problem, as Program::RemoveFixedBlocks does). */
+ *  - The call leaves the handle's SubsetManifolds (b200_set_subset_manifolds) alone.
+ * B200_ERR_INVALID_ARGUMENT, with the handle unchanged: h == NULL, or a row whose camera and point are both constant,
+ * a full SubsetManifold counting as constant (Ceres moves such a row's cost into fixed_cost; drop the row from the
+ * problem, as Program::RemoveFixedBlocks does). */
 int b200_set_constant_blocks(b200_handle* h, const uint8_t* camera_constant, const uint8_t* point_constant);
+/* Problem::SetManifold(block, new SubsetManifold(n, S)) for every block at once: single coordinates held constant.
+   camera_constant_coordinates[C]: bit k (k < 9) set = coordinate k of the camera [angle-axis | t | f, k1, k2] is
+   constant, i.e. SubsetManifold(9, {k : bit k}); point_constant_coordinates[P], bits k < 3, likewise for the points of
+   this shard, in the caller's order.  0 = no SubsetManifold on that block; NULL = none on any block of that kind.
+ * The call replaces the handle's masks from the next evaluation on; the set of constant blocks
+ * (b200_set_constant_blocks) stays as it is, and each block's effective state is the union of both, as in Ceres, where
+ * SetParameterBlockConstant and SetManifold are independent.  A full mask (tangent size 0) makes its block constant
+ * (ParameterBlock::IsConstant) with every consequence described above.  A masked coordinate of a variable block is held
+ * as a constant block's components are -- zero Jacobian column, D' = 1 in every solve, exact zeros in every solution, x
+ * kept bitwise by b200_plus and b200_lm_solve, the stored J's cells zeroed by the call and after
+ * b200_jacobian_set_values -- with three differences, which follow Ceres:
+ *  - Evaluation checks the ambient Jacobian before it drops the masked columns (residual_block.cc:85-159): a non-finite
+ *    value in a masked column fails the evaluation, where in a constant block's column it does not.
+ *  - b200_lm_solve's |x| for parameter_tolerance counts masked coordinates: Ceres' reduced x is the ambient state of the
+ *    variable blocks (trust_region_minimizer.cc:725-734).
+ *  - b200_covariance_cameras / _points lift the tangent covariance with the plus Jacobian (covariance_impl.cc:240-265):
+ *    masked rows and columns of a block are 0, and masked coordinates take no part in the conditioning test.
+ * The layout stays [3P | 9C]: S keeps 9 x 9 camera blocks, with identity rows on masked coordinates, so fixing
+ * intrinsics does not make the exact solves cheaper.  Sharded handles: each rank passes its own points' masks and the
+ * same camera masks.
+ * B200_ERR_INVALID_ARGUMENT, with the handle unchanged: h == NULL, a camera mask with bits above 8 or a point mask with
+ * bits above 2, or a row whose camera and point are then both constant. */
+int b200_set_subset_manifolds(b200_handle* h, const uint16_t* camera_constant_coordinates, const uint8_t* point_constant_coordinates);
 /* Evaluator::Plus (evaluator.h:146; Euclidean manifolds only): x_plus_delta = x + delta. */
 int b200_plus(b200_handle* h, const double* x, const double* delta, double* x_plus_delta);
 
