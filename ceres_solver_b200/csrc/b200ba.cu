@@ -541,23 +541,14 @@ int sqnorm_dev(b200_handle* h, double* d_out);
 // The evaluate kernels of the plan for one class of loss set (loss.cuh); *num_partials = the per-tile / per-CTA cost
 // partials they wrote.
 template <int kLoss, bool kFixed>
-int evaluate_launch(b200_handle* h, EvalArgs a, const double* d_gradient, bool want_jacobian, double* d_sqnorm,
-                    bool* sqnorm_done, int* num_partials) {
-  const bool with_j = want_jacobian || d_gradient != nullptr;
+int evaluate_launch(b200_handle* h, EvalArgs a, bool want_jacobian, double* d_sqnorm, bool* sqnorm_done, int* num_partials) {
+  const bool with_j = want_jacobian || a.gradient != nullptr;
   const size_t coff = 3 * static_cast<size_t>(h->P);
   const size_t smem = tile_smem_bytes<3, 1>();
   *num_partials = h->num_tiles;
   if (with_j && is_v4(h->mul)) {
-    EvalV2Args e{};
-    e.state = a.state;
-    e.residuals = a.residuals;
-    e.gradient = a.gradient;
-    e.sqnorm = d_sqnorm;
-    e.cost_partial = h->d_tile_partial;
-    e.scale = a.scale;
-    e.fail_flag = h->d_fail;
-    e.loss = a.loss;
-    e.block_state = a.block_state;
+    EvalArgs e = a;
+    e.sqnorm = d_sqnorm;   // the CTA-tile kernel below leaves them to sqnorm_kernel
     if (d_sqnorm != nullptr) CU(cudaMemsetAsync(d_sqnorm + coff, 0, sizeof(double) * 9 * h->C, h->stream));
     if (d_sqnorm != nullptr) OK(huge_zero(h, d_sqnorm));
     OK(launch(h, K_EVAL_JAC, [&] {
@@ -593,10 +584,16 @@ int evaluate_launch(b200_handle* h, EvalArgs a, const double* d_gradient, bool w
   return B200_OK;
 }
 template <int kLoss>
-int evaluate_launch(b200_handle* h, EvalArgs a, const double* d_gradient, bool want_jacobian, double* d_sqnorm,
-                    bool* sqnorm_done, int* num_partials) {
-  if (h->fixed_any) return evaluate_launch<kLoss, true>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, num_partials);
-  return evaluate_launch<kLoss, false>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, num_partials);
+int evaluate_launch(b200_handle* h, EvalArgs a, bool want_jacobian, double* d_sqnorm, bool* sqnorm_done, int* num_partials) {
+  if (h->fixed_any) return evaluate_launch<kLoss, true>(h, a, want_jacobian, d_sqnorm, sqnorm_done, num_partials);
+  return evaluate_launch<kLoss, false>(h, a, want_jacobian, d_sqnorm, sqnorm_done, num_partials);
+}
+
+// What a write of the stored J makes stale: the explicit S and the per-row blocks Q_r of the implicit-Schur
+// initialisation.  The initialisation itself stays: the b200_schur_* entry points keep using its (E'E + D^2)^-1.
+void jacobian_written(b200_handle* h) {
+  h->xs_ready = false;
+  h->q_from_init = false;
 }
 
 // d_sqnorm (optional): squared column norms of the Jacobian as written (after the fused scaling), for free with the
@@ -606,7 +603,7 @@ int evaluate_launch(b200_handle* h, EvalArgs a, const double* d_gradient, bool w
 int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, double* d_gradient, bool want_jacobian,
                  const double* d_scale, double* cost_out, double* d_sqnorm = nullptr, bool* sqnorm_done = nullptr) {
   if (!want_jacobian) d_sqnorm = nullptr;   // the column norms are those of the stored Jacobian
-  else h->xs_ready = false;                 // S is a function of J
+  else jacobian_written(h);
   EvalArgs a{};
   a.state = d_state;
   a.residuals = d_residuals;
@@ -626,9 +623,9 @@ int evaluate_dev(b200_handle* h, const double* d_state, double* d_residuals, dou
   if (d_gradient != nullptr) OK(huge_zero(h, d_gradient));
   int num_partials = 0;
   switch (h->apply_loss ? h->loss_cls : kLossTrivial) {
-    case kLossTrivial: OK(evaluate_launch<kLossTrivial>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
-    case kLossHuber: OK(evaluate_launch<kLossHuber>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
-    default: OK(evaluate_launch<kLossGeneral>(h, a, d_gradient, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
+    case kLossTrivial: OK(evaluate_launch<kLossTrivial>(h, a, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
+    case kLossHuber: OK(evaluate_launch<kLossHuber>(h, a, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
+    default: OK(evaluate_launch<kLossGeneral>(h, a, want_jacobian, d_sqnorm, sqnorm_done, &num_partials)); break;
   }
   OK(launch(h, K_MISC, [&] { sum_kernel<<<1, kVecThreads, 0, h->stream>>>(num_partials, h->d_tile_partial, h->d_scalars); }));
   if (d_gradient != nullptr) OK(allreduce_sum(h, d_gradient + 3 * static_cast<size_t>(h->P), 9 * static_cast<size_t>(h->C)));
@@ -662,14 +659,14 @@ int sqnorm_dev(b200_handle* h, double* d_out) {
 // Zeroes the stored Jacobian's cells of the handle's constant components (none: nothing to do).
 int fixed_mask_dev(b200_handle* h) {
   if (!h->fixed_any) return B200_OK;
-  h->xs_ready = false;   // S is a function of J
+  jacobian_written(h);
   return launch(h, K_SCALE, [&] {
     fixed_mask_kernel<<<flat_grid(h, 12 * static_cast<size_t>(h->N), 256), 256, 0, h->stream>>>(h->view, h->d_fixed);
   }, false);
 }
 
 int scale_dev(b200_handle* h, const double* d_scale) {
-  h->xs_ready = false;   // S is a function of J
+  jacobian_written(h);
   return launch(h, K_SCALE, [&] {
     scale_kernel<<<flat_grid(h, 12 * static_cast<size_t>(h->N), 256), 256, 0, h->stream>>>(h->view, d_scale);
   });
@@ -2471,11 +2468,10 @@ int set_fixed(b200_handle* h, std::vector<uint8_t> cam_const, std::vector<uint8_
   h->fixed_any = st.any;
   OK(fixed_mask_dev(h));
   CU(cudaStreamSynchronize(h->stream));   // (the uploads read st, which goes out of scope)
-  // everything formed from J is stale: the explicit S, the Schur initialisation and the preconditioner built on it
-  h->xs_ready = false;
+  // everything formed from J is stale, the Schur initialisation and the preconditioner built on it included
+  jacobian_written(h);
   h->xs_diag_ready = false;
   h->schur_ready = false;
-  h->q_from_init = false;
   return B200_OK;
 }
 
@@ -3260,7 +3256,7 @@ int b200_jacobian_get_values(b200_handle* h, double* values) {
 int b200_jacobian_set_values(b200_handle* h, const double* values) {
   if (h == nullptr || values == nullptr) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
   CU(cudaSetDevice(h->device));
-  h->xs_ready = false;   // S is a function of J
+  jacobian_written(h);
   const size_t n = static_cast<size_t>(h->N);
   if (!h->permuted) {
     OK(h2d(h, h->d_values, values, sizeof(double) * 24 * n));
@@ -3353,10 +3349,9 @@ int b200_covariance_compute(b200_handle* h, const double* state, const b200_cova
   bool factored = false;
   int rc = dense ? cov_dense_dev(h, &factored) : cov_sparse_dev(h, &factored);
   // the Schur initialisation, S and the factor now hold the covariance's: the next solve rebuilds them
+  jacobian_written(h);
   h->schur_ready = false;
-  h->xs_ready = false;
   h->xs_diag_ready = false;
-  h->q_from_init = false;
   OK(rc);
   if (!factored) {
     if (getenv("B200_VERBOSE") != nullptr) fprintf(stderr, "[b200ba] covariance: S is not positive definite\n");

@@ -85,27 +85,15 @@ __host__ __device__ constexpr int upper9_col(int idx) {
   return a + idx;
 }
 
-struct EvalV2Args {
-  const double* state;
-  double* residuals;     // [2N] or null
-  double* gradient;      // [3P+9C] or null; camera part zeroed by the caller
-  double* sqnorm;        // [3P+9C] or null; camera part zeroed by the caller: squared column norms of the WRITTEN Jacobian
-  double* cost_partial;  // [num_ctas]
-  const double* scale;   // null or [3P+9C]
-  int* fail_flag;
-  LossArgs loss;
-  const uint16_t* block_state;  // [P + C], kFixed only (evaluate_kernel)
-};
-
 constexpr int kEvalScratch = 3;  // doubles per lane in the exchange scratch
 __host__ __device__ inline int eval_v2_per_warp_bytes() { return 32 * 144 + 32 * 48 + 32 * kEvalScratch * 8; }
 
 // Evaluate residuals, Jacobian (written through a per-warp staging buffer + TMA bulk store), cost, gradient and the
 // squared column norms of the Jacobian as written (i.e. after the fused Jacobi scaling).
 // kStoreJ = false (gradient without the Jacobian): as evaluate_kernel<kLoss, true, false>, the Jacobian is left as it is.
-// kFixed: constant blocks' cells and coordinates held by a SubsetManifold are 0, as in evaluate_kernel.
+// kFixed: constant blocks' cells and coordinates held by a SubsetManifold are 0 (evaluate_row).
 template <int kLoss, bool kStoreJ, bool kFixed = false>
-__global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v, EvalV2Args a) {
+__global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v, EvalArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int2 part = v.cta_part[blockIdx.x];
@@ -138,28 +126,9 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
     for (int k = 0; k < 18; ++k) jc[k] = 0.0;
 #pragma unroll
     for (int k = 0; k < 6; ++k) jp[k] = 0.0;
-    size_t po = 0;
-    if (active) {
-      po = 3 * static_cast<size_t>(wt.pt_begin + sg.lpt);
-      const double* cp = a.state + camoff + 9 * static_cast<size_t>(cam);
-      const double2 o = *reinterpret_cast<const double2*>(v.p.obs + 2 * row);
-      snavely<true>(cp, a.state[po], a.state[po + 1], a.state[po + 2], o.x, o.y, r0, r1, jc, jp);
-      uint32_t mp = 0, mc = 0;
-      if (kFixed) {
-        mp = __ldg(a.block_state + wt.pt_begin + sg.lpt);
-        mc = __ldg(a.block_state + v.p.P + cam);
-        constant_cells(mp, mc, jc, jp);
-      }
-      bool finite = isfinite(r0) && isfinite(r1);
-#pragma unroll
-      for (int k = 0; k < 18; ++k) finite = finite && isfinite(jc[k]);
-#pragma unroll
-      for (int k = 0; k < 6; ++k) finite = finite && isfinite(jp[k]);
-      if (!finite) atomicExch(a.fail_flag, 1);
-      if (kFixed) masked_cells(mp, mc, jc, jp);
-      cost += apply_loss<kLoss, true>(row_loss_entry<kLoss>(a.loss, row), r0, r1, jc, jp);
-      if (a.residuals != nullptr) *reinterpret_cast<double2*>(a.residuals + 2 * row) = make_double2(r0, r1);
-    }
+    const int pt = wt.pt_begin + sg.lpt;
+    const size_t po = 3 * static_cast<size_t>(pt);
+    if (active) cost += evaluate_row<kLoss, true, kFixed>(v.p, a, row, wt.pt_begin, sg.lpt, cam, r0, r1, jc, jp);
     // gradient of the unscaled Jacobian (program_evaluator.h:242-259)
     if (a.gradient != nullptr) {
       double gp[3], gps[3], gc[9];
@@ -176,21 +145,7 @@ __global__ void __launch_bounds__(kV2MaxThreads, 1) evaluate_v2_kernel(V2View v,
       if (owned) cam_accumulate9_owned(my_g, cam_l, active, gc);   // one private copy per warp: plain read-modify-write
       else cam_accumulate<9>(my_g, cam_l, active, gc);
     }
-    if (a.scale != nullptr && active) {
-      const double* sc = a.scale + camoff + 9 * static_cast<size_t>(cam);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const double s = a.scale[po + k];
-        jp[k] *= s;
-        jp[3 + k] *= s;
-      }
-#pragma unroll
-      for (int k = 0; k < 9; ++k) {
-        const double s = sc[k];
-        jc[k] *= s;
-        jc[9 + k] *= s;
-      }
-    }
+    if (a.scale != nullptr && active) scale_row(a.scale, v.p.P, pt, cam, jc, jp);
     if (a.sqnorm != nullptr) {
       double qp[3], qps[3], qc[9];
 #pragma unroll

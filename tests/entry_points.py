@@ -132,6 +132,24 @@ def check_every_entry_point(case, oracle, shared_inputs=False):
         xd, _, td = gpu.dense_schur_solve(res, D)
         xdo, _, tdo = J.linear_solve(P, res_o, D, solver=1, nt=8)
         assert td == tdo and relerr(xd, xdo) < 1e-7
+    # SCHUR_JACOBI after a write of J that no new initialisation followed: every configuration forms the blocks from the
+    # current J and the initialisation's P = (E'E + D_e^2)^-1, F'F + D_f^2 - sum_k W_kc' P_k W_kc with W_kc the sum of
+    # E_r'F_r over the rows of point k and camera c
+    gpu.schur_init(res, D)
+    Pk = gpu.schur_ete_inverse().reshape(P, 3, 3)
+    gpu.scale_columns(rng.uniform(0.5, 2.0, gpu.num_parameters))
+    v = gpu.jacobian_values()
+    N = gpu.N
+    E, F = v[:6 * N].reshape(N, 2, 3), v[6 * N:].reshape(N, 2, 9)
+    cam, pt = np.asarray(case.rp.row_cam), np.asarray(case.rp.row_pt)
+    expect = np.einsum("ci,ij->cij", D[3 * P:].reshape(C, 9) ** 2, np.eye(9))
+    np.add.at(expect, cam, np.einsum("nri,nrj->nij", F, F))
+    pairs, pair_of_row = np.unique(pt.astype(np.int64) * C + cam, return_inverse=True)
+    W = np.zeros((pairs.size, 3, 9))
+    np.add.at(W, pair_of_row.ravel(), np.einsum("nri,nrj->nij", E, F))
+    np.subtract.at(expect, pairs % C, np.einsum("kij,kil,klm->kjm", W, Pk[pairs // C], W))
+    blocks, _ = gpu.schur_jacobi_update()
+    assert relerr(blocks, expect.ravel()) < 1e-9
 
 
 def oracle_lm_traces(case, iterations, max_cg=None, threads=(8, 3)):

@@ -82,10 +82,10 @@ def threshold_between(fire, before):
     return t
 
 
-def exit_values(orc, state, recs, name):
+def exit_values(orc, state, recs, name, nt=8):
     """{iteration: value} of what the exit `name` compares with its option at each iteration of the oracle trace `recs`
     (trust_region_minimizer.cc: the gradient and radius tests on every record, :316-361; the parameter and function
-    tolerances on every valid candidate, :726-769)."""
+    tolerances on every valid candidate, :726-769).  nt: the oracle's threads for the solves it runs."""
     if name == "gradient_tolerance":
         return {int(r["iteration"]): r["gradient_max_norm"] for r in recs if r["step_is_successful"]}
     if name == "min_trust_region_radius":
@@ -98,21 +98,22 @@ def exit_values(orc, state, recs, name):
             if name == "function_tolerance":
                 out[j] = abs(r["cost_change"]) / x_cost
             elif accepted:   # parameter_tolerance: |step| / |x|, tested once a step has been accepted
-                x, _, _ = oracle_solve(orc, state, max_num_iterations=j - 1)   # x at iteration j (the best state so far)
+                x, _, _ = oracle_solve(orc, state, nt=nt, max_num_iterations=j - 1)   # x at iteration j (the best so far)
                 out[j] = r["step_norm"] / np.linalg.norm(x)
         if r["step_is_successful"]:
             x_cost, accepted = r["cost"], True
     return out
 
 
-def place_exit(orc, state, name, k, base=None):
+def place_exit(orc, state, name, k, base=None, nt=8):
     """(options, number of records) of a solve on which exit `name` fires at iteration k: the threshold comes from the
     oracle's run with `base` options (default ones if None) and no exit before iteration k + 1.  The gradient and radius
-    exits end the loop after record k is written, the parameter and function tolerances before it."""
+    exits end the loop after record k is written, the parameter and function tolerances before it.  nt: the oracle's
+    threads."""
     base = dict(base or {})
     base["max_num_iterations"] = k + 1
-    _, recs, _ = oracle_solve(orc, state, **base)
-    values = exit_values(orc, state, recs, name)
+    _, recs, _ = oracle_solve(orc, state, nt=nt, **base)
+    values = exit_values(orc, state, recs, name, nt)
     t = threshold_between(values[k], [v for j, v in values.items() if j < k])
     if name == "parameter_tolerance":
         # the test is |step| <= t (|x| + t): t^2 against t |x| moves the threshold by t / |x|, a tenth of MARGIN at most

@@ -1,10 +1,11 @@
 """The Huber loss (bundle_adjuster --robustify) in every evaluate kernel, against the oracle.
 
-The loss and its corrector are applied in two copies of the same code: evaluate_v2_kernel (warp tiles, points of up to
-32 rows, Jacobian wanted) and evaluate_kernel<kWantJ> (CTA tiles: every cost-only evaluate, points of more than 32 rows,
-and every row in the configurations without warp-tile evaluate).  Each problem here sets the Huber parameter a to its
-median row norm at the initial state, so that every class of rows (points of <= 32, 33..128 and > 128 rows) has inliers
-and outliers and both branches of every copy run; tests/test_oracle_lm_control.py asserts that on a CPU machine.
+The loss and its corrector are applied by one row function (evaluate_row) in two kernels: evaluate_v2_kernel (warp
+tiles, points of up to 32 rows, Jacobian wanted) and evaluate_kernel<kWantJ> (CTA tiles: every cost-only evaluate,
+points of more than 32 rows, and every row in the configurations without warp-tile evaluate).  Each problem here sets
+the Huber parameter a to its median row norm at the initial state, so that every class of rows (points of <= 32,
+33..128 and > 128 rows) has inliers and outliers and both branches run in both kernels; tests/test_oracle_lm_control.py
+asserts that on a CPU machine.
 
   - every entry point (tests/entry_points.py) on the fixtures of tests/test_gpu_dispatch.py, C16 and the huge-point
     problem of tests/test_gpu_parity.py: evaluate with and without the Jacobian against the oracle (cost 1e-12, Jacobian

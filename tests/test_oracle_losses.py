@@ -362,9 +362,11 @@ def test_huber_against_the_oracle(oracle, c16):
             assert relerr(lp.jacobian().values(), orc.jacobian().values()) < 1e-15
             if name == "tiny":
                 continue   # tiny converges in four iterations, to cost changes at the rounding level of its cost
+            # one thread: threaded, the Schur elimination adds into shared blocks in lock order, and the distance of
+            # the two programs' DENSE_SCHUR solutions moves from run to run across the bound on x below
             for solver in (L.ITERATIVE_SCHUR, L.DENSE_SCHUR):
-                x_o, recs_o, _ = L.oracle_solve(orc, state, max_num_iterations=5, linear_solver_type=solver)
-                x, recs, _ = L.oracle_solve(lp, state, max_num_iterations=5, linear_solver_type=solver)
+                x_o, recs_o, _ = L.oracle_solve(orc, state, nt=1, max_num_iterations=5, linear_solver_type=solver)
+                x, recs, _ = L.oracle_solve(lp, state, nt=1, max_num_iterations=5, linear_solver_type=solver)
                 compare_lm_traces_exact(recs, recs_o)
                 assert relerr(x, x_o) < 1e-12
 
